@@ -385,6 +385,83 @@ def fuzz_trace(n: int, num_blocks: int, *, block_size: int = 512, seed: int = 1,
     return t
 
 
+# ------------------------------------------------------------------------------------------------
+# Alignment sweep: the byte-granular movers (lun_kernel.cuh move_unit_unaligned / _compact, lun_kernel.cu
+# move_unit_via_smem) at every skew and at the lengths where their cases change.  Deterministic.
+# ------------------------------------------------------------------------------------------------
+
+PIECE_BODY = 2032        # lun_kernel.cu kPieceBody: a staged unit's first piece ends at head + 2032 bytes
+
+
+def sweep_lengths(dst_skew: int) -> list[int]:
+    """element lengths at the movers' edges for a destination at `dst_skew` (mod 16): under / at / over one
+    vector; just below, at and just above the staged-piece split (head + 2032: second piece empty, empty, one
+    byte); one unit -1 / 0 / +1; and a run of four units with an odd tail"""
+    p = (16 - dst_skew) % 16 + PIECE_BODY
+    return [1, 15, 16, 17, p - 1, p, p + 1, 4095, 4096, 4097, 3 * 4096 + 1234]
+
+
+def alignment_sweep(num_blocks: int = 65536, *, block_size: int = 512, target: int = 0, per_request: int = 32) -> Trace:
+    """READs and WRITEs whose SG elements sweep (client address mod 16) x (store offset mod 16) x sweep_lengths,
+    followed by two passes of misaligned READs behind WRITEs to the same blocks (same pass, next pass).
+
+    Every element has a client buffer of its own (no element continues another, so each is one segment of the
+    mover).  The store offset of an element is set by the elements before it in its request: a spacer element
+    brings it to the wanted value mod 16, and a last element pads the request to whole blocks.  WRITEs go to the
+    first half of the device, READs read the second, the hazard passes use the last 1024 blocks."""
+    assert block_size % 16 == 0
+    b = abi.Batch(target)
+    cursor = [0]
+
+    def buf(n: int, skew: int) -> int:
+        o = (cursor[0] + 127) // 64 * 64 + skew        # >= 64 bytes past the previous buffer's end
+        cursor[0] = o + n
+        return o
+
+    lba = {abi.DIR_TO_DEV: 0, abi.DIR_FROM_DEV: num_blocks // 2}
+    for d in (abi.DIR_FROM_DEV, abi.DIR_TO_DEV):
+        read = d == abi.DIR_FROM_DEV
+        cases = [(c, s, n) for c in range(16) for s in range(16) for n in sweep_lengths(c if read else s)]
+        for k in range(0, len(cases), per_request):
+            els, store = [], 0
+            for j, (c, s, n) in enumerate(cases[k:k + per_request]):
+                gap = (s - store) % 16 + 16 * (j % 3)
+                if gap:
+                    els.append((buf(gap, (c + 7) % 16), gap))
+                    store += gap
+                els.append((buf(n, c), n))
+                store += n
+            pad = -store % block_size
+            if pad:
+                els.append((buf(pad, 9), pad))
+                store += pad
+            nblk = store // block_size
+            if read:
+                b.read(lba[d], nblk, els)
+            else:
+                b.write(lba[d], nblk, els)
+            lba[d] += nblk
+    hz = num_blocks - 1024
+    assert lba[abi.DIR_TO_DEV] <= num_blocks // 2 and lba[abi.DIR_FROM_DEV] <= hz, "num_blocks too small for the sweep"
+    while len(b._reqs) % abi.REQS_PER_PASS:                  # the hazard passes start on a pass boundary
+        b.read(hz + 512 + len(b._reqs) % 8, 1, [(buf(512, 0), 512)])
+    for g in range(8):                                       # pass p: W, R (RAW), R (RAW, part), W (WAW, WAR)
+        x = hz + 16 * g
+        b.write(x, 8, [(buf(100 + g, (3 + g) % 16), 100 + g), (buf(3996 - g, (11 + g) % 16), 3996 - g)])
+        b.read(x, 8, [(buf(4096, (5 + 2 * g) % 16), 4096)])
+        b.read(x + 1, 2, [(buf(333, (g + 1) % 16), 333), (buf(691, (2 * g + 3) % 16), 691)])
+        b.write(x + 4, 2, [(buf(1024, (13 + g) % 16), 1024)])
+    for g in range(8):                                       # pass p + 1: reads of what pass p wrote, one more write
+        x = hz + 16 * g
+        b.read(x, 8, [(buf(4096, (5 * g + 1) % 16), 4096)])
+        b.read(x + 3, 4, [(buf(7, (g + 9) % 16), 7), (buf(2033, (g + 2) % 16), 2033), (buf(0, 0), 0),
+                          (buf(8, (15 - g) % 16), 8)])
+        b.write(x + 7, 1, [(buf(512, (g + 6) % 16), 512)])
+        b.read(x + 6, 2, [(buf(1024, (3 * g + 7) % 16), 1024)])
+    reqs, iovs = b.arrays()
+    return Trace(reqs, iovs, cursor[0] + 4096, "alignment-sweep", {"hazard_pass": len(reqs) // abi.REQS_PER_PASS - 2})
+
+
 def _param_iovs(alloc, payload: np.ndarray, rng) -> list[tuple[int, int]]:
     """SG list for a TO_DEV parameter list (UNMAP): one element, or cut in two at a ragged spot."""
     n = len(payload)

@@ -16,25 +16,25 @@ from test_oracle import GOLDEN, bdevio_cases, load_golden, run_bdevio  # noqa: F
 pytestmark = pytest.mark.gpu
 
 
-@pytest.mark.parametrize("path", GOLDEN, ids=[os.path.basename(p) for p in GOLDEN])
-@pytest.mark.parametrize("mem", ["device", "host"])
-def test_cuda_matches_reference_golden_vectors(gpu, path, mem):
+@pytest.mark.parametrize("kernel,mem,path", util.kernel_cases([(m, p) for p in GOLDEN for m in ("device", "host")],
+                                                                ids=lambda v: f"{v[0]}-{os.path.basename(v[1])}"))
+def test_cuda_matches_reference_golden_vectors(gpu, path, mem, kernel):
     t, z = load_golden(path)
-    cpls, arena, store, _ = util.run_cuda(gpu, t, int(z["num_blocks"]), mem=mem, removed=bool(z["removed"]))
-    util.assert_cpls_equal(cpls, z["cpls"], t.reqs, f"cuda[{mem}]:{t.name}")
+    cpls, arena, store, _ = util.run_cuda(gpu, t, int(z["num_blocks"]), mem=mem, removed=bool(z["removed"]), kernel=kernel)
+    util.assert_cpls_equal(cpls, z["cpls"], t.reqs, f"cuda[{kernel}, {mem}]:{t.name}")
     assert util.sha(arena) == str(z["arena_sha"]), "client buffers differ from the reference's"
     assert util.sha(store) == str(z["store_sha"]), "backing store differs from the reference's"
 
 
-@pytest.mark.parametrize("seed", range(300, 316))
-def test_cuda_matches_oracle_on_fuzz(gpu, oracles, seed):
+@pytest.mark.parametrize("kernel,seed", util.kernel_cases(range(300, 316), range(300, 304)))
+def test_cuda_matches_oracle_on_fuzz(gpu, oracles, kernel, seed):
     """fresh seeded traces: all opcodes, ragged/unaligned/empty SG lists, limits, malformed requests,
     with a hot spot so that RAW/WAW/WAR hazards inside a 32-request pass are common"""
     nb = 32768
     t = traces.fuzz_trace(500, nb, seed=seed, max_io_blocks=[8, 64, 300, 1024][seed % 4],
                           arena_bytes=(8 << 20) if seed % 4 < 3 else (48 << 20))
     want = util.run_oracle(oracles.PortOracle, t, nb)
-    got = util.run_cuda(gpu, t, nb, mem="device" if seed % 2 else "host")
+    got = util.run_cuda(gpu, t, nb, mem="device" if seed % 2 else "host", kernel=kernel)
     util.assert_cpls_equal(got[0], want[0], t.reqs, f"seed {seed}")
     assert (got[1] == want[1]).all(), f"client arena differs at {np.nonzero(got[1] != want[1])[0][:8]}"
     assert (got[2] == want[2]).all(), f"store differs at {np.nonzero(got[2] != want[2])[0][:8]}"
@@ -44,8 +44,8 @@ def test_cuda_matches_oracle_on_fuzz(gpu, oracles, seed):
         assert (got[1] == ref[1]).all() and (got[2] == ref[2]).all()
 
 
-@pytest.mark.parametrize("seed", range(340, 348))
-def test_cuda_sg_elements_that_continue_each_other(gpu, oracles, seed):
+@pytest.mark.parametrize("kernel,seed", util.kernel_cases(range(340, 348), range(340, 344)))
+def test_cuda_sg_elements_that_continue_each_other(gpu, oracles, kernel, seed):
     """SG lists cut from ONE client buffer at arbitrary bytes (with zero-length elements and gaps in between): the
     kernel moves a run of elements that continue each other in client memory as one segment (lun_kernel.cu
     parse_request / emit_segments), the reference copies element by element (bdev_malloc.c:180-189) - same bytes"""
@@ -54,14 +54,23 @@ def test_cuda_sg_elements_that_continue_each_other(gpu, oracles, seed):
                           arena_bytes=(8 << 20) if seed % 4 < 3 else (48 << 20))
     checker = oracles.RefOracle if oracles.ref_available() and seed % 2 else oracles.PortOracle
     want = util.run_oracle(checker, t, nb)
-    got = util.run_cuda(gpu, t, nb, mem="device" if seed % 2 else "host")
+    got = util.run_cuda(gpu, t, nb, mem="device" if seed % 2 else "host", kernel=kernel)
     util.assert_cpls_equal(got[0], want[0], t.reqs, f"seed {seed}")
     assert (got[1] == want[1]).all(), f"client arena differs at {np.nonzero(got[1] != want[1])[0][:8]}"
     assert (got[2] == want[2]).all(), f"store differs at {np.nonzero(got[2] != want[2])[0][:8]}"
 
 
 def test_cuda_hazards_same_lba_chain(gpu, oracles):
-    """32 requests of one pass all on the same blocks: W,R,W,R,... must serialise exactly"""
+    """32 requests of one pass all on the same blocks: W,R,W,R,... must serialise exactly (shared kernel)"""
+    _hazards_same_lba_chain(gpu, oracles, "shared")
+
+
+@pytest.mark.parametrize("kernel", util.OTHER_KERNELS)
+def test_cuda_hazards_same_lba_chain_on(gpu, oracles, kernel):
+    _hazards_same_lba_chain(gpu, oracles, kernel)
+
+
+def _hazards_same_lba_chain(gpu, oracles, kernel):
     nb = 4096
     b = abi.Batch(0)
     off = 64
@@ -74,13 +83,13 @@ def test_cuda_hazards_same_lba_chain(gpu, oracles):
     reqs, iovs = b.arrays()
     t = traces.Trace(reqs, iovs, off + 4096, "chain")
     want = util.run_oracle(oracles.PortOracle, t, nb)
-    got = util.run_cuda(gpu, t, nb)
+    got = util.run_cuda(gpu, t, nb, kernel=kernel)
     util.assert_cpls_equal(got[0], want[0], t.reqs)
     assert (got[1] == want[1]).all() and (got[2] == want[2]).all()
 
 
-@pytest.mark.parametrize("shape", ["hot4k", "sub_granule", "mixed_sizes"])
-def test_cuda_hazard_signatures(gpu, oracles, shape):
+@pytest.mark.parametrize("kernel,shape", util.kernel_cases(["hot4k", "sub_granule", "mixed_sizes"]))
+def test_cuda_hazard_signatures(gpu, oracles, kernel, shape):
     """the signature filter in front of the exact range check (lun_kernel.cu): conflicts in nearly every pass
     (hot4k), requests that share a 4 KiB granule without overlapping and with overlapping (sub_granule),
     and requests from one block to more than the signature's granule limit (mixed_sizes)"""
@@ -105,7 +114,7 @@ def test_cuda_hazard_signatures(gpu, oracles, shape):
     t = traces.Trace(reqs, iovs, off + 4096, shape)
     want = util.run_oracle(oracles.PortOracle, t, nb)
     for _ in range(2):
-        got = util.run_cuda(gpu, t, nb)
+        got = util.run_cuda(gpu, t, nb, kernel=kernel)
         util.assert_cpls_equal(got[0], want[0], t.reqs)
         assert (got[1] == want[1]).all(), f"client memory differs at {np.nonzero(got[1] != want[1])[0][:8]}"
         assert (got[2] == want[2]).all(), f"store differs at {np.nonzero(got[2] != want[2])[0][:8]}"
@@ -113,7 +122,18 @@ def test_cuda_hazard_signatures(gpu, oracles, shape):
 
 def test_cuda_hazards_two_passes_apart(gpu, oracles):
     """movers are not in lock-step: while one is still busy with a 4 MiB write of pass p, the others run
-    through pass p+1 (unrelated small reads) and reach pass p+2, which reads what pass p writes"""
+    through pass p+1 (unrelated small reads) and reach pass p+2, which reads what pass p writes.  Shared kernel:
+    the passes usually land on different CTAs."""
+    _hazards_two_passes_apart(gpu, oracles, "shared")
+
+
+@pytest.mark.parametrize("kernel", util.OTHER_KERNELS)
+def test_cuda_hazards_two_passes_apart_on(gpu, oracles, kernel):
+    """exclusive / mirror: one CTA runs the three passes back to back (waves, drain between passes)"""
+    _hazards_two_passes_apart(gpu, oracles, kernel)
+
+
+def _hazards_two_passes_apart(gpu, oracles, kernel):
     nb = 1 << 16
     b = abi.Batch(0)
     off = 4096
@@ -135,19 +155,56 @@ def test_cuda_hazards_two_passes_apart(gpu, oracles):
     t = traces.Trace(reqs, iovs, off + 4096, "two-apart")
     want = util.run_oracle(oracles.PortOracle, t, nb)
     for _ in range(3):
-        got = util.run_cuda(gpu, t, nb)
+        got = util.run_cuda(gpu, t, nb, kernel=kernel)
         util.assert_cpls_equal(got[0], want[0], t.reqs)
         assert (got[1] == want[1]).all(), "a read overtook the write two passes ahead of it"
         assert (got[2] == want[2]).all()
 
 
 def test_cuda_non_pow2_block_size(gpu, oracles):
+    _non_pow2_block_size(gpu, oracles, "shared")
+
+
+@pytest.mark.parametrize("kernel", util.OTHER_KERNELS)
+def test_cuda_non_pow2_block_size_on(gpu, oracles, kernel):
+    _non_pow2_block_size(gpu, oracles, kernel)
+
+
+def _non_pow2_block_size(gpu, oracles, kernel):
     nb, bs = 9000, 520
     t = traces.fuzz_trace(300, nb, block_size=bs, seed=77, max_io_blocks=16)
     want = util.run_oracle(oracles.PortOracle, t, nb, block_size=bs)
-    got = util.run_cuda(gpu, t, nb, block_size=bs)
+    got = util.run_cuda(gpu, t, nb, block_size=bs, kernel=kernel)
     util.assert_cpls_equal(got[0], want[0], t.reqs)
     assert (got[1] == want[1]).all() and (got[2] == want[2]).all()
+
+
+def _element_at(t, off: int) -> str:
+    """which SG element of the trace covers arena offset `off` (for failure messages)"""
+    a, n = t.iovs["addr"].astype(np.int64), t.iovs["len"].astype(np.int64)
+    hit = np.nonzero((a <= off) & (off < a + n))[0]
+    if not len(hit):
+        return f"arena byte {off}: in no element (a neighbour was overwritten)"
+    j = int(hit[0])
+    r = int(np.nonzero((t.reqs["iov_start"] <= j) & (j < t.reqs["iov_start"].astype(np.int64) + t.reqs["iovcnt"]))[0][0])
+    return f"arena byte {off}: request {r}, element {j} (address mod 16 = {a[j] % 16}, length {n[j]}, byte {off - a[j]})"
+
+
+@pytest.mark.parametrize("kernel,mem", util.kernel_cases(["device", "host"], ["device"]))
+def test_cuda_alignment_sweep(gpu, oracles, kernel, mem):
+    """traces.alignment_sweep through every variant: each (client, store) skew at the byte-granular movers' edge
+    lengths (staged pieces, realign cases, prefetched units, the compact path of the mirror kernels) and misaligned
+    reads behind writes in the same and the next pass.  The whole client arena and the whole store are compared:
+    both hold position-keyed pseudo-random bytes, so a misplaced byte or a stray write next to a buffer shows."""
+    nb = 65536
+    t = traces.alignment_sweep(nb)
+    want = util.run_oracle(oracles.PortOracle, t, nb)
+    got = util.run_cuda(gpu, t, nb, mem=mem, kernel=kernel)
+    util.assert_cpls_equal(got[0], want[0], t.reqs, f"sweep[{kernel}, {mem}]")
+    bad = np.nonzero(got[1] != want[1])[0]
+    assert not len(bad), f"client memory differs at {len(bad)} bytes; first: {_element_at(t, int(bad[0]))}"
+    bad = np.nonzero(got[2] != want[2])[0]
+    assert not len(bad), f"store differs at {len(bad)} bytes, first at byte {bad[:8]}"
 
 
 class DevBuf:
@@ -506,27 +563,68 @@ def test_cuda_control_plane_errors(gpu):
     gpu.load().oimgpu_set_socket_dir(b"", None)
 
 
+COPY_LENGTHS = [1, 15, 16, 17, 2031, 2032, 2033, 2047, 2048, 2049, 4095, 4096, 4097, 3 * 4096 + 1234]
+BIG = (5 << 20) + 13                                        # several units per warp and an odd tail
+
+
+def _slots(cases, n_of):
+    """one slot per case in one buffer: 64 guard bytes, the case's range at its offset mod 16, 64 guard bytes"""
+    base, out = 0, []
+    for c in cases:
+        out.append(base + 64)
+        base += (64 + 16 + n_of(c) + 64 + 63) // 64 * 64
+    return out, base
+
+
 def test_cuda_copy_engine_level(gpu):
-    """B2: struct spdk_copy_engine {copy, fill} on device buffers, odd sizes and alignments"""
+    """B2: struct spdk_copy_engine {copy, fill} on device buffers.  copy: every (destination, source) offset mod 16
+    (the 16 realign16 skews of move_unit_unaligned, each with every destination head) at the lengths where the mover's
+    cases change, plus a few of several MiB; fill: every destination offset.  The cases sit side by side in one
+    buffer between guard bytes of a pseudo-random pattern, and the WHOLE buffer is compared with a numpy replay:
+    a wrong byte, a byte out of place or a store past either end of a range fails."""
     import torch
     gpu.construct_malloc_bdev(2048, 512, name="ce0", device=0)
     gpu.construct_vhost_scsi_controller("ce.ctl")
     gpu.add_vhost_scsi_lun("ce.ctl", 0, "ce0")
     try:
         with gpu.Lun("ce.ctl", 0) as lun:
-            src = torch.randint(0, 256, (5 << 20,), dtype=torch.uint8, device="cuda:0")
-            dst = torch.zeros_like(src)
+            # copy: (dst offset, src offset, length)
+            cases = [(do, so, n) for n in COPY_LENGTHS for do in range(16) for so in range(16)]
+            cases += [(0, 0, BIG), (1, 0, BIG), (0, 1, BIG), (3, 11, BIG), (15, 15, BIG), (15, 2, BIG)]
+            at, size = _slots(cases, lambda c: c[2])
+            src_h = traces.pattern_bytes(0xC0, 0, size).copy()
+            dst_h = traces.pattern_bytes(0xD5, 0, size).copy()
+            src, dst = torch.from_numpy(src_h).to("cuda:0"), torch.from_numpy(dst_h).to("cuda:0")
             torch.cuda.synchronize()
-            for (do, so, n) in [(0, 0, 5 << 20), (1, 3, 100003), (16, 32, 4096), (5, 5, 17), (7, 0, 1)]:
-                dst.zero_()
-                torch.cuda.synchronize()
-                lun.copy(dst.data_ptr() + do, src.data_ptr() + so, n)
-                lun.sync()
-                assert torch.equal(dst[do:do + n], src[so:so + n]), (do, so, n)
-                assert int(dst[do + n:do + n + 64].sum()) == 0 and int(dst[:do].sum()) == 0
-                lun.fill(dst.data_ptr() + do, 0xAB, n)
-                lun.sync()
-                assert bool((dst[do:do + n] == 0xAB).all()) and int(dst[do + n:do + n + 64].sum()) == 0
+            want = dst_h.copy()
+            for (do, so, n), o in zip(cases, at):
+                lun.copy(dst.data_ptr() + o + do, src.data_ptr() + o + so, n)
+                want[o + do:o + do + n] = src_h[o + so:o + so + n]
+            lun.sync()
+            got = dst.cpu().numpy()
+            bad = np.nonzero(got != want)[0]
+            if len(bad):
+                k = max(0, int(np.searchsorted(np.asarray(at) - 64, bad[0], side="right")) - 1)
+                raise AssertionError(f"copy: {len(bad)} bytes differ; first at byte {int(bad[0]) - at[k]} of the slot of "
+                                     f"(dst mod 16, src mod 16, length) = {cases[k]}")
+            assert (src.cpu().numpy() == src_h).all(), "copy wrote into its source"
+            # fill: (dst offset, length, value)
+            cases = [(do, n, (37 * i + 1) & 0xFF) for i, (do, n) in
+                     enumerate((do, n) for n in COPY_LENGTHS + [BIG] for do in range(16))]
+            at, size = _slots(cases, lambda c: c[1])
+            dst_h = traces.pattern_bytes(0xF1, 0, size).copy()
+            dst = torch.from_numpy(dst_h).to("cuda:0")
+            torch.cuda.synchronize()
+            want = dst_h.copy()
+            for (do, n, v), o in zip(cases, at):
+                lun.fill(dst.data_ptr() + o + do, v, n)
+                want[o + do:o + do + n] = v
+            lun.sync()
+            bad = np.nonzero(dst.cpu().numpy() != want)[0]
+            if len(bad):
+                k = max(0, int(np.searchsorted(np.asarray(at) - 64, bad[0], side="right")) - 1)
+                raise AssertionError(f"fill: {len(bad)} bytes differ; first at byte {int(bad[0]) - at[k]} of the slot of "
+                                     f"(dst mod 16, length, value) = {cases[k]}")
     finally:
         gpu.remove_vhost_scsi_target("ce.ctl", 0)
         gpu.remove_vhost_controller("ce.ctl")

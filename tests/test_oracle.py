@@ -53,6 +53,20 @@ def test_restatement_matches_reference_on_fresh_fuzz(oracles, seed):
     assert (got[1] == want[1]).all() and (got[2] == want[2]).all()
 
 
+def test_restatement_matches_reference_on_alignment_sweep(oracles):
+    """traces.alignment_sweep: every (client, store) skew at the byte-granular movers' edge lengths, and misaligned
+    reads behind writes; the GPU variants are compared with the restatement on it (test_gpu_parity.py)"""
+    if not oracles.ref_available():
+        pytest.skip("oracle/_ref not built here (no /root/reference)")
+    nb = 65536
+    t = traces.alignment_sweep(nb)
+    want = util.run_oracle(oracles.RefOracle, t, nb)
+    got = util.run_oracle(oracles.PortOracle, t, nb)
+    util.assert_cpls_equal(got[0], want[0], t.reqs, "alignment sweep")
+    assert (got[1] == want[1]).all() and (got[2] == want[2]).all()
+    assert (want[0]["status"] == 0).all(), "every request of the sweep is a good one"
+
+
 # ---- known-answer cases of the reference's own unit tests ------------------------------------
 
 def _one(o, cdb, direction, iovs):

@@ -22,8 +22,9 @@ def _oracle(oracles, t, nb, seed=7):
     return cpls, arena, store
 
 
-def _run_batch(gpu, name, t, nb, nq, per_q, seed=7):
-    """one oimgpu_submit_batch launch: queue q <- requests [q*per_q, (q+1)*per_q), everything in HBM"""
+def _run_batch(gpu, name, t, nb, nq, per_q, seed=7, kernel="shared"):
+    """one oimgpu_submit_batch launch: queue q <- requests [q*per_q, (q+1)*per_q), everything in HBM.
+    kernel="exclusive": with OIMGPU_NO_SHARED_QUEUES=1 (one CTA per queue)"""
     import torch
     gpu.construct_malloc_bdev(nb, 512, name=name, device=0)
     gpu.construct_vhost_scsi_controller(name + ".ctl")
@@ -37,11 +38,12 @@ def _run_batch(gpu, name, t, nb, nq, per_q, seed=7):
         d_iovs = torch.from_numpy(t.bind(dev.data_ptr()).view(np.uint8).copy()).cuda()
         d_cpls = torch.zeros(len(t.reqs) * 48, dtype=torch.uint8, device="cuda")
         torch.cuda.synchronize()
-        with gpu.Lun(name + ".ctl", 0, num_queues=nq, queue_size=32) as lun:
+        with util.environ(**util.kernel_env(kernel)), gpu.Lun(name + ".ctl", 0, num_queues=nq, queue_size=32) as lun:
             lun.submit_batch(nq, per_q, d_reqs.data_ptr(), d_iovs.data_ptr(), len(t.iovs), d_cpls.data_ptr(), abi.MEM_DEVICE)
             lun.sync()
             shared = lun.shared_launches
             stats = lun.iostat()
+        assert stats["kernel_launches"] == 1
         cpls = np.frombuffer(d_cpls.cpu().numpy().tobytes(), dtype=abi.cpl_dtype)
         return cpls, dev.cpu().numpy(), gpu.bdev_read_raw(name, 0, nb * 512), shared, stats
     finally:
@@ -77,16 +79,17 @@ def test_shared_queues_match_sequential_result(gpu, oracles, nq, per_q, read_pct
     assert got[4]["num_read_ops"] == reads and got[4]["num_write_ops"] == nq * per_q - reads
 
 
-@pytest.mark.parametrize("seed", [31, 32, 33])
-def test_shared_queue_fuzz_every_opcode(gpu, oracles, seed):
-    """the adversarial trace (UNMAP, control payloads, malformed requests, ragged SG lists) on ONE queue in one launch"""
+@pytest.mark.parametrize("kernel,seed", util.kernel_cases([31, 32, 33], kernels=("shared", "exclusive")))
+def test_shared_queue_fuzz_every_opcode(gpu, oracles, seed, kernel):
+    """the adversarial trace (UNMAP, control payloads, malformed requests, ragged SG lists) on ONE queue in one launch:
+    shared by the CTAs a pass at a time, and (exclusive) the whole queue on one CTA"""
     nb = 1 << 15
     t = traces.fuzz_trace(3000, nb, seed=seed, max_io_blocks=96, arena_bytes=64 << 20)
     n = len(t.reqs) // 32 * 32
     t = traces.Trace(t.reqs[:n].copy(), t.iovs, t.arena_bytes, t.name, t.meta)
     want = _oracle(oracles, t, nb)
-    got = _run_batch(gpu, f"shfz{seed}", t, nb, 1, n)
-    assert got[3] == 1
+    got = _run_batch(gpu, f"shfz{seed}{kernel}", t, nb, 1, n, kernel=kernel)
+    assert got[3] == (kernel == "shared"), f"the launch did not take the {kernel} path"
     util.assert_cpls_equal(got[0], want[0], t.reqs)
     assert (got[1] == want[1]).all() and (got[2] == want[2]).all()
 

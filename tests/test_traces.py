@@ -2,7 +2,7 @@
 import numpy as np
 
 import util
-from oim_b200 import traces, vring
+from oim_b200 import abi, traces, vring
 
 
 def continues(iov):
@@ -55,6 +55,44 @@ def test_fuzz_traces_with_runs_of_contiguous_elements(oracles):
         util.assert_cpls_equal(want[0], ref[0], runs.reqs, "runs")
         assert (want[1] == ref[1]).all() and (want[2] == ref[2]).all()
     assert (want[0]["status"] == 0).sum() > 200
+
+
+def test_alignment_sweep_covers_every_skew_and_edge(oracles):
+    """traces.alignment_sweep: every (client address mod 16, store offset mod 16, edge length) for READ and WRITE, each
+    element its own segment, whole blocks per request; then a pass that reads and rewrites what it writes, and a pass
+    that reads it back"""
+    nb = 65536
+    t = traces.alignment_sweep(nb)
+    seen = {abi.DIR_FROM_DEV: set(), abi.DIR_TO_DEV: set()}
+    lbas = []
+    for r in t.reqs:
+        iov = t.iovs[int(r["iov_start"]):int(r["iov_start"]) + int(r["iovcnt"])]
+        assert 0 < len(iov) <= 129
+        cdb = bytes(r["cdb"])
+        assert cdb[0] in (abi.READ_10, abi.WRITE_10)
+        lba, nblk = int.from_bytes(cdb[2:6], "big"), int.from_bytes(cdb[7:9], "big")
+        assert int(iov["len"].sum()) == nblk * 512 and lba + nblk <= nb
+        assert not continues(iov[iov["len"] > 0]).any(), "an element continues another: they would be one segment"
+        store = 0
+        for a, n in zip(iov["addr"], iov["len"]):
+            seen[int(r["dir"])].add((int(a) % 16, store % 16, int(n)))
+            store += int(n)
+        lbas.append((lba, nblk, int(r["dir"])))
+    for d in seen:
+        for c in range(16):
+            for s in range(16):
+                dst = c if d == abi.DIR_FROM_DEV else s
+                for n in traces.sweep_lengths(dst):
+                    assert (c, s, n) in seen[d], (d, c, s, n)
+    # the staged unit's piece split (lun_kernel.cu piece0_bytes): second piece empty at and below head + 2032
+    assert {n - (16 - 3) % 16 - traces.PIECE_BODY for n in traces.sweep_lengths(3)} >= {-1, 0, 1}
+    p = t.meta["hazard_pass"] * abi.REQS_PER_PASS
+    assert p % abi.REQS_PER_PASS == 0 and len(t.reqs) == p + 2 * abi.REQS_PER_PASS
+    w, r = lbas[p], lbas[p + 1]
+    assert w[2] == abi.DIR_TO_DEV and r[2] == abi.DIR_FROM_DEV and w[:2] == r[:2], "pass p: a read behind a write"
+    assert lbas[p + abi.REQS_PER_PASS][:2] == w[:2], "pass p + 1: a read of what pass p wrote"
+    cpls = util.run_oracle(oracles.PortOracle, t, nb)[0]
+    assert (cpls["status"] == 0).all() and (cpls["resid"] == 0).all(), "every request of the sweep is a good one"
 
 
 def test_guest_images_with_runs_of_contiguous_descriptors():

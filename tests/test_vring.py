@@ -3,7 +3,17 @@ CPU: the C restatement against the compiled reference.  GPU: the kernel's own ri
 import numpy as np
 import pytest
 
+import util
 from oim_b200 import traces, vring
+
+# the kernels that serve a virtqueue-only kick, and the environment that selects each (liboimgpu.so launch_lun_kernel)
+VQ_KERNELS = {
+    "shared": {"OIMGPU_NO_SHARED_QUEUES": None, "OIMGPU_SHARE_MAX_QUEUES": None, "OIMGPU_NO_VRING_KERNEL": None},
+    # oim_lun_vring_kernel: one CTA per queue, the register realign path (move_unit_unaligned)
+    "vring": {"OIMGPU_NO_SHARED_QUEUES": "1", "OIMGPU_NO_VRING_KERNEL": None},
+    # oim_lun_queue_kernel in virtqueue mode: what a kick that mixes virtqueues and slot rings runs
+    "queue": {"OIMGPU_NO_SHARED_QUEUES": "1", "OIMGPU_NO_VRING_KERNEL": "1"},
+}
 
 
 def make_requests(seed: int, n: int = 96, nb: int = 32768, contiguous: bool = False):
@@ -57,11 +67,13 @@ def test_vring_broken_avail_index(oracles):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("seed", list(range(420, 432)) + [1420, 1421, 1422, 1423])
-@pytest.mark.parametrize("mem", ["device", "host"])
-def test_cuda_vring_matches_oracle(gpu, oracles, seed, mem):
+@pytest.mark.parametrize("kernel,mem,seed", util.kernel_cases(
+    [(m, s) for s in list(range(420, 432)) + [1420, 1421, 1422, 1423] for m in ("device", "host")],
+    ids=lambda v: f"{v[0]}-{v[1]}", kernels=list(VQ_KERNELS)))
+def test_cuda_vring_matches_oracle(gpu, oracles, seed, mem, kernel):
     """seeds >= 1000: every request's data descriptors are cuts of one guest buffer - the kernel moves a run of
-    descriptors that continue each other as one segment, the reference copies them one by one"""
+    descriptors that continue each other as one segment, the reference copies them one by one.  Every kick is one
+    launch of `kernel` (the guest buffers sit at random byte offsets: the byte-granular movers of each)."""
     import torch
     contiguous = seed >= 1000
     nb, rq = 32768, make_requests(seed, contiguous=contiguous)
@@ -69,12 +81,13 @@ def test_cuda_vring_matches_oracle(gpu, oracles, seed, mem):
     checker = oracles.RefOracle if oracles.ref_available() and seed % 2 else oracles.PortOracle
     want, want_store = run_kicks_oracle(checker, rq, nb, ring, seed, contiguous=contiguous)
 
-    gpu.construct_malloc_bdev(nb, 512, name=f"vq{seed}{mem}", device=0)
-    gpu.construct_vhost_scsi_controller(f"vq{seed}{mem}.ctl")
-    gpu.add_vhost_scsi_lun(f"vq{seed}{mem}.ctl", 0, f"vq{seed}{mem}")
+    name = f"vq{seed}{mem}{kernel}"
+    gpu.construct_malloc_bdev(nb, 512, name=name, device=0)
+    gpu.construct_vhost_scsi_controller(f"{name}.ctl")
+    gpu.add_vhost_scsi_lun(f"{name}.ctl", 0, name)
     try:
-        gpu.bdev_write_raw(f"vq{seed}{mem}", 0, traces.pattern_bytes(7, 0, nb * 512))
-        with gpu.Lun(f"vq{seed}{mem}.ctl", 0, num_queues=2, queue_size=32) as lun:
+        gpu.bdev_write_raw(name, 0, traces.pattern_bytes(7, 0, nb * 512))
+        with util.environ(**VQ_KERNELS[kernel]), gpu.Lun(f"{name}.ctl", 0, num_queues=2, queue_size=32) as lun:
             pos = kick = 0
             la = lu = 0
             while pos < len(rq):
@@ -87,8 +100,10 @@ def test_cuda_vring_matches_oracle(gpu, oracles, seed, mem):
                 base = dev.data_ptr()
                 lun.set_mem_table(img.region_table(base))
                 lun.vq_attach(1, base + img.desc_off, base + img.avail_off, base + img.used_off, img.ring_size, 0, 0)
+                shared = lun.shared_launches
                 assert lun.vq_kick() == 1
                 lun.sync()
+                assert lun.shared_launches - shared == (kernel == "shared"), f"kick {kick} did not take the {kernel} kernel"
                 la, lu = lun.vq_detach(1)
                 after = dev.cpu().numpy() if mem == "device" else dev.numpy().copy()
                 idx, uring = img.used_entries(after)
@@ -101,8 +116,9 @@ def test_cuda_vring_matches_oracle(gpu, oracles, seed, mem):
                 assert [int(i) for i in uring[:idx]["id"]] == img.heads[:idx]
                 pos += img.meta["placed"]
                 kick += 1
-        assert (gpu.bdev_read_raw(f"vq{seed}{mem}", 0, nb * 512) == want_store).all()
+            assert lun.iostat()["kernel_launches"] == kick, "one launch per kick"
+        assert (gpu.bdev_read_raw(name, 0, nb * 512) == want_store).all()
     finally:
-        gpu.remove_vhost_scsi_target(f"vq{seed}{mem}.ctl", 0)
-        gpu.remove_vhost_controller(f"vq{seed}{mem}.ctl")
-        gpu.delete_bdev(f"vq{seed}{mem}")
+        gpu.remove_vhost_scsi_target(f"{name}.ctl", 0)
+        gpu.remove_vhost_controller(f"{name}.ctl")
+        gpu.delete_bdev(name)
