@@ -167,7 +167,7 @@ __device__ __forceinline__ void ustage_consume(uint8_t *dst, const uint8_t *src,
  * async proxy: the first staged unit after such a barrier crosses proxies with a fence.  Prefetched units never
  * follow a barrier (the mover asks for the next unit only when nothing has to be waited for in between).
  * nsrc != nullptr: the unit this warp moves next, (ndst, nsrc, nn), also takes this path - request it. */
-__device__ OIM_SMEM_PATH_INLINE void move_unit_via_smem(uint8_t *dst, const uint8_t *src, uint32_t n, int lane,
+__device__ __forceinline__ void move_unit_via_smem(uint8_t *dst, const uint8_t *src, uint32_t n, int lane,
 							  uint8_t *ust, uint64_t *bar, UStage &us, bool &pfence,
 							  uint8_t *ndst, const uint8_t *nsrc, uint32_t nn)
 {
@@ -1251,6 +1251,403 @@ __device__ __forceinline__ uint32_t find_shared_work(const KickHeader *hdr, cons
 #ifndef OIM_MIN_BLOCKS
 #define OIM_MIN_BLOCKS 2	/* 128 registers: the mover loop must stay spill-free (a lower register cap spills it) */
 #endif
+
+/* every mover has finished fill f (a mover arrives on `empty` only after finishing its share of all earlier fills too) */
+__device__ __forceinline__ void wait_fill_moved(CtaShared &sh, uint32_t f)
+{
+	mbar_wait(&sh.empty[f % kStages], (f / kStages) & 1);
+}
+
+/* ---- the dispatcher CTA (see KickHeader) --------------------------------------------------------------- */
+
+/* one warp: mirror every queue's doorbell into VqState::hint, and the stop flag into stop_mirror */
+__device__ __forceinline__ void dispatcher_cta(KickHeader *hdr, const QueueDesc *queues, int lane)
+{
+	const uint32_t nq = hdr->nqueues;
+	uint64_t last_change = globaltimer_ns();
+	for (;;) {
+		bool changed = false;
+		for (uint32_t base = 0; base < nq; base += 32) {
+			const uint32_t qi = base + lane;
+			if (qi < nq) {
+				const QueueDesc &q = queues[qi];
+				const uint32_t v = q.mode == QMODE_VRING ? (uint32_t)ld_vol16(q.vq_avail + 2) : ld_vol32(q.doorbell);
+				if (v != ld_vol32(&q.vq_state->hint)) {
+					st_vol32(&q.vq_state->hint, v);
+					changed = true;
+				}
+			}
+		}
+		changed = __any_sync(0xffffffffu, changed);
+		uint32_t quit = 0;
+		if (lane == 0) {
+			const uint64_t now = globaltimer_ns();
+			if (changed) last_change = now;
+			quit = ld_vol32(hdr->stop) != 0;
+			if (!quit && hdr->idle_timeout_ms && now - last_change > (uint64_t)hdr->idle_timeout_ms * 1000000ull) quit = 1;
+			if (quit) st_vol32(&hdr->stop_mirror, 1u);
+		}
+		if (__shfl_sync(0xffffffffu, quit, 0)) break;
+	}
+	if (lane == 0) {
+		__threadfence_system();
+		atomicAdd_system(const_cast<uint32_t *>(hdr->exited), 1u);
+	}
+}
+
+/* ---- parser: one pass ---------------------------------------------------------------------------------- */
+
+struct PassHazards {
+	uint32_t writers, touching;	/* lane masks of the pass: haz >= 2, haz != 0 */
+	uint32_t drain;			/* 0 = none, d = fill c-d must be finished before flagged units move */
+	bool cross;			/* this lane's request is one of the conflicting ones */
+	bool mydense;			/* its range is too large (or a barrier) for the signatures */
+	bool wcollide;			/* a writer found one of its granules already written in this pass */
+	uint64_t g0, g1;		/* its first and last 4 KiB granule */
+};
+
+/* Hazards against the passes whose movers may still be running.  The history ring hist[] keeps the store ranges of
+ * the previous kStages-1 passes per lane: movers are not in lock-step, one may already work on pass p+2 while another
+ * is still in pass p (the stage ring only stops the parser from refilling pass p's stage).  The segments of a request
+ * that conflicts with one of them are flagged; a mover that reaches a flagged unit first waits until the conflicting
+ * fill is finished, everything else in the pass proceeds at once.  (Waiting for fill c-d's `empty` barrier covers all
+ * older ones too.)  Records this pass in hist[pass_no % kStages]. */
+__device__ __forceinline__ PassHazards cross_pass_hazards(HazPass *hist, uint32_t pass_no, uint32_t haz, uint64_t lo, uint64_t hi, int lane)
+{
+	constexpr int kHist = kStages - 1;
+	PassHazards r;
+	r.drain = 0;
+	r.cross = false;
+	r.writers = __ballot_sync(0xffffffffu, haz >= 2);
+	r.touching = __ballot_sync(0xffffffffu, haz != 0);
+	HazPass &cur = hist[pass_no % kStages];
+	/* a read-only stream never needs signatures: while neither this pass nor the ones it could be compared with
+	 * contain a writer, the pass is left unsigned (= "dense": whoever meets it later falls back to the exact ranges) */
+	bool sign = r.writers != 0;
+#pragma unroll
+	for (int h = 1; h <= kHist; h++) {
+		if ((uint32_t)h <= pass_no) sign |= hist[(pass_no - h) % kStages].writers != 0;
+	}
+	if (sign) {
+		for (int k = lane; k < kSigWords; k += 32) { cur.sig_r[k] = 0; cur.sig_w[k] = 0; }
+	}
+	cur.lo[lane] = lo;
+	cur.hi[lane] = hi;
+	cur.haz[lane] = (uint8_t)haz;
+	if (lane == 0) { cur.writers = r.writers; cur.touching = r.touching; cur.dense = sign ? 0 : 1; }
+	__syncwarp();
+	r.g0 = lo >> 12;
+	r.g1 = haz ? (hi - 1) >> 12 : r.g0;
+	r.mydense = haz == 3 || (haz && r.g1 - r.g0 >= (uint64_t)kSigMaxGranules);
+	r.wcollide = false;
+	if (!sign) { /* nothing to publish */ }
+	else if (r.mydense) cur.dense = 1;
+	else if (haz) {
+		for (uint64_t g = r.g0; g <= r.g1; g++) {
+			const uint32_t idx = sig_index(g);
+			if (haz >= 2) r.wcollide |= (atomicOr(&cur.sig_w[idx >> 5], 1u << (idx & 31)) >> (idx & 31)) & 1u;
+			else atomicOr(&cur.sig_r[idx >> 5], 1u << (idx & 31));
+		}
+	}
+	__syncwarp();
+	/* against the kStages-1 passes before this one: signature first, exact ranges only for the requests the signature
+	 * cannot clear */
+#pragma unroll
+	for (int h = kHist; h >= 1; h--) {
+		if ((uint32_t)h > pass_no) continue;
+		const HazPass &pp = hist[(pass_no - h) % kStages];
+		const uint32_t candidates = haz >= 2 ? pp.touching : haz ? pp.writers : 0u;
+		bool maybe = false;
+		if (candidates) {
+			if (r.mydense || pp.dense) maybe = true;
+			else {
+				for (uint64_t g = r.g0; g <= r.g1; g++) {
+					const uint32_t idx = sig_index(g);
+					uint32_t word = pp.sig_w[idx >> 5];
+					if (haz >= 2) word |= pp.sig_r[idx >> 5];
+					maybe |= (word >> (idx & 31)) & 1u;
+				}
+			}
+		}
+		bool hit = false;
+		if (maybe) {
+			uint32_t scan = candidates;
+			while (scan) {
+				const int j = __ffs(scan) - 1;
+				scan &= scan - 1;
+				if (haz == 3 || pp.haz[j] == 3 || (lo < pp.hi[j] && pp.lo[j] < hi)) hit = true;
+			}
+		}
+		r.cross |= hit;
+		if (__any_sync(0xffffffffu, hit)) r.drain = (uint32_t)h;	/* nearest pass wins */
+	}
+	return r;
+}
+
+/* Hazards inside the pass -> waves.  Writers are visited in ring order; a writer is pushed behind every earlier
+ * request it overlaps, every later overlapping request behind the writer.  Most passes have no overlap at all: the
+ * signatures say so.  Returns this lane's wave and the pass's number of waves in nwaves. */
+__device__ __forceinline__ uint16_t assign_waves(const HazPass &cur, const PassHazards &hz, uint32_t haz, uint64_t lo, uint64_t hi,
+						 int lane, uint32_t &nwaves)
+{
+	uint16_t wave = 0;
+	nwaves = 1;
+	bool inpass = false;
+	if (hz.writers && (hz.touching & (hz.touching - 1)) && haz) {
+		if (hz.mydense || cur.dense) inpass = true;
+		else if (haz >= 2) {
+			inpass = hz.wcollide;
+			for (uint64_t g = hz.g0; g <= hz.g1; g++) {
+				const uint32_t idx = sig_index(g);
+				inpass |= (cur.sig_r[idx >> 5] >> (idx & 31)) & 1u;
+			}
+		} else {
+			for (uint64_t g = hz.g0; g <= hz.g1; g++) {
+				const uint32_t idx = sig_index(g);
+				inpass |= (cur.sig_w[idx >> 5] >> (idx & 31)) & 1u;
+			}
+		}
+	}
+	if (!__any_sync(0xffffffffu, inpass)) return wave;
+	uint32_t w = hz.writers;
+	while (w) {
+		const int j = __ffs(w) - 1;
+		w &= w - 1;
+		const uint64_t jlo = __shfl_sync(0xffffffffu, lo, j);
+		const uint64_t jhi = __shfl_sync(0xffffffffu, hi, j);
+		const uint32_t jhaz = __shfl_sync(0xffffffffu, haz, j);
+		const bool overlap = haz != 0 && lane != j &&
+			(jhaz == 3 || haz == 3 || (lo < jhi && jlo < hi));
+		uint32_t need = (overlap && lane < j) ? (uint32_t)wave + 1 : 0;
+		need = __reduce_max_sync(0xffffffffu, need);
+		if (lane == j && need > wave) wave = (uint16_t)need;
+		const uint32_t jw = __shfl_sync(0xffffffffu, (uint32_t)wave, j);
+		if (overlap && lane > j && jw + 1 > wave) wave = (uint16_t)(jw + 1);
+	}
+	nwaves = __reduce_max_sync(0xffffffffu, (uint32_t)wave) + 1;
+	return wave;
+}
+
+/* counters for get_bdevs_iostat, per parser lane; one atomic per counter per CTA when the parser leaves */
+struct IoStats {
+	uint32_t rd = 0, wr = 0, um = 0, er = 0;
+	uint32_t mix_r = 0, mix_w = 0;		/* good reads / writes + unmaps of ANY target: the session's mix */
+	unsigned long long rb = 0, wb = 0, ub = 0;
+
+	/* good: the request completed with GOOD status */
+	__device__ __forceinline__ void count(const LunCtx &L, const LaneState &s, bool active, bool good)
+	{
+		const bool own = !good || s.tgt == L.target;	/* failures are booked on the session's device */
+		const bool ok = good && own;
+		rd += __popc(__ballot_sync(0xffffffffu, ok && s.op == OP_READ));
+		wr += __popc(__ballot_sync(0xffffffffu, ok && s.op == OP_WRITE));
+		/* UNMAP reaches the bdev once per applied descriptor, whatever the command's final status */
+		const bool unmapped = active && s.resp_valid && s.response == OIMGPU_S_OK && s.op == OP_UNMAP && s.tgt == L.target;
+		um += __reduce_add_sync(0xffffffffu, unmapped ? s.nseg : 0u);
+		if (unmapped) ub += s.unmap_bytes;
+		er += __popc(__ballot_sync(0xffffffffu, active && !good));
+		mix_r += __popc(__ballot_sync(0xffffffffu, good && s.op == OP_READ));
+		mix_w += __popc(__ballot_sync(0xffffffffu, good && (s.op == OP_WRITE || s.op == OP_UNMAP)));
+		if (ok && s.op == OP_READ) rb += s.length;
+		if (ok && s.op == OP_WRITE) wb += s.length;
+		if (active && s.resp_valid && s.response == OIMGPU_S_OK && s.tgt != L.target &&
+		    ((good && (s.op == OP_READ || s.op == OP_WRITE)) || s.op == OP_UNMAP)) {
+			/* another device of the controller: book it there (rare path, plain atomics) */
+			LunCtx *P = L.peer[s.tgt];
+			if (s.op == OP_UNMAP) {
+				if (s.nseg) { atomicAdd(&P->stats[2], (unsigned long long)s.nseg); atomicAdd(&P->stats[6], (unsigned long long)s.unmap_bytes); }
+			} else {
+				const int k = s.op == OP_READ ? 0 : 1;
+				atomicAdd(&P->stats[k], 1ull);
+				atomicAdd(&P->stats[4 + k], (unsigned long long)s.length);
+			}
+		}
+	}
+
+	/* every fill is retired: mover warp 0 is done adding to sh.lat_ns */
+	__device__ __forceinline__ void flush(LunCtx *lun, const CtaShared &sh, int lane)
+	{
+		for (int o = 16; o; o >>= 1) {
+			rb += __shfl_xor_sync(0xffffffffu, rb, o);
+			wb += __shfl_xor_sync(0xffffffffu, wb, o);
+			ub += __shfl_xor_sync(0xffffffffu, ub, o);
+		}
+		if (lane != 0) return;
+		if (ub) atomicAdd(&lun->stats[6], ub);
+		if (rd) { atomicAdd(&lun->stats[0], (unsigned long long)rd); atomicAdd(&lun->stats[4], rb); }
+		if (wr) { atomicAdd(&lun->stats[1], (unsigned long long)wr); atomicAdd(&lun->stats[5], wb); }
+		if (um) atomicAdd(&lun->stats[2], (unsigned long long)um);
+		if (er) atomicAdd(&lun->stats[7], (unsigned long long)er);
+		if (mix_r) atomicAdd(&lun->mix[0], (unsigned long long)mix_r);
+		if (mix_w) atomicAdd(&lun->mix[1], (unsigned long long)mix_w);
+		for (int t = 0; t < OIMGPU_CTRLR_MAX_DEVS; t++) {
+			LunCtx *T = (t == lun->target) ? lun : lun->peer[t];
+			for (int k = 0; k < 3 && T; k++) {
+				if (sh.lat_ns[t][k]) atomicAdd(&T->stats[8 + k], sh.lat_ns[t][k]);
+			}
+		}
+	}
+};
+
+/* ---- movers -------------------------------------------------------------------------------------------- */
+
+/* the fill a mover warp works through */
+struct MoverFill {
+	const Stage &st;
+	uint32_t nseg, nunits, nw;
+
+	/* the segment that holds unit u: the last one with first_unit <= u */
+	__device__ __forceinline__ const Segment &seg_of(uint32_t u) const
+	{
+		uint32_t lo = u, hi = nseg;
+		/* as many units as segments: segment u IS unit u.  Taken for passes of small requests (the 4 KiB case); long
+		 * SG lists of single pages keep the search - the lookup's latency spreads the movers' loads there */
+		if (nunits != nseg || nseg > (uint32_t)kPass) {
+			lo = 0;
+			while (hi - lo > 1) {
+				const uint32_t mid = (lo + hi) >> 1;
+				if (st.seg[mid].first_unit <= u) lo = mid; else hi = mid;
+			}
+		}
+		return st.seg[lo];
+	}
+};
+
+/* the unit a mover warp takes after u: every kMovers-th, or (dyn) the next one from the fill's counter */
+__device__ __forceinline__ uint32_t next_unit(Stage &st, bool dyn, uint32_t u, int lane)
+{
+	if (!dyn) return u + kMovers;
+	uint32_t v = 0;
+	if (lane == 0) v = atomicAdd(&st.unit_ctr, 1u);
+	return __shfl_sync(0xffffffffu, v, 0);
+}
+
+/* Unit u of segment g: mirror fan-out, zero fill, aligned copy, or a byte-granular copy - in registers (mirror and
+ * vring kernels) or, in the staged kernels, through this warp's staging buffer with the next unit requested early */
+template <bool kMirrored, bool kStaged>
+__device__ __forceinline__ void move_seg_unit(const LunCtx *lun, const MoverFill &f, const Segment &g, uint32_t u, uint32_t u_next,
+					      uint32_t w, bool drained, int lane, uint8_t *ust, uint64_t *ubar, UStage &us, bool &upfence)
+{
+	const uint64_t off = (uint64_t)(u - g.first_unit) * kUnitBytes;
+	const uint32_t nbytes = (uint32_t)min((uint64_t)kUnitBytes, g.len - off);
+	const uint8_t *src = g.src;
+	uint8_t *dst = g.dst;
+	if (kMirrored && g.mirror) {
+		const LunCtx &T = (g.mirror - 1 == lun->target) ? *lun : *lun->peer[g.mirror - 1];
+		mirror_unit(T, dst, src, off, nbytes, lane, T.nreplicas);
+	} else if (!src) {
+		zero_unit(dst + off, nbytes, lane);
+	} else if constexpr (kMirrored) {
+		move_unit<true>(dst + off, src + off, nbytes, lane);
+	} else if ((((uintptr_t)(dst + off) | (uintptr_t)(src + off) | nbytes) & 15) == 0) {
+		move_unit(dst + off, src + off, nbytes, lane);
+	} else if constexpr (!kStaged) {
+		move_unit(dst + off, src + off, nbytes, lane);
+	} else {
+		/* the unit this warp moves next, when it is known and nothing has to be waited for before it may be read:
+		 * its bytes are requested while this one is realigned */
+		uint8_t *ndst = nullptr; const uint8_t *nsrc = nullptr; uint32_t nn = 0;
+		if (u_next < f.nunits) {
+			const Segment &g2 = f.seg_of(u_next);
+			if (g2.src && (f.nw == 1 || (g2.wave & kSegWaveMask) == w) && (!(g2.wave & kSegWaitsForDrain) || drained)) {
+				const uint64_t off2 = (uint64_t)(u_next - g2.first_unit) * kUnitBytes;
+				nn = (uint32_t)min((uint64_t)kUnitBytes, g2.len - off2);
+				if ((((uintptr_t)(g2.dst + off2) | (uintptr_t)(g2.src + off2) | nn) & 15) != 0) { ndst = g2.dst + off2; nsrc = g2.src + off2; }
+			}
+		}
+		move_unit_via_smem(dst + off, src + off, nbytes, lane, ust, ubar, us, upfence, ndst, nsrc, nn);
+	}
+}
+
+/* mover warp 0, lane 0: the fill's data has moved - add its latency to the sums and histograms of its targets */
+__device__ __forceinline__ void tally_fill_latency(CtaShared &sh, const Stage &st, const LunCtx *lun)
+{
+	const unsigned long long dt = globaltimer_ns() - st.t0;
+	for (uint32_t i = 0; i < st.lat_ntgt; i++) {
+		const uint32_t t = st.lat_tgt[i] & (OIMGPU_CTRLR_MAX_DEVS - 1);
+		unsigned long long *acc = sh.lat_ns[t];
+		acc[0] += dt * st.lat_n[i][0]; acc[1] += dt * st.lat_n[i][1]; acc[2] += dt * st.lat_n[i][2];
+		/* spdk_histogram_data_tally (histogram_data.h:120-160) of the fill's latency, once per request */
+		const LunCtx *T = (t == lun->target) ? lun : lun->peer[t];
+		unsigned long long *hist = T ? *reinterpret_cast<unsigned long long *const volatile *>(&T->hist) : nullptr;
+		if (hist && dt) {
+			const uint32_t clz = (uint32_t)__clzll((long long)dt);
+			const uint32_t range = clz <= 57u ? 57u - clz : 0u;
+			const uint32_t index = (uint32_t)(dt >> (range ? range - 1 : 0)) & 127u;
+			atomicAdd(&hist[(range << 7) + index], (unsigned long long)(st.lat_n[i][0] + st.lat_n[i][1] + st.lat_n[i][2]));
+		}
+	}
+}
+
+/* ======================= MOVERS (warps 1..kMovers) ======================= */
+template <bool kMirrored, bool kMoverReap, bool kStaged>
+__device__ __forceinline__ void mover_warp(CtaShared &sh, const LunCtx *lun, int mw, int lane)
+{
+	UStage us = {nullptr, 0};	/* this warp's staging buffer (move_unit_via_smem) */
+	bool upfence = true;		/* the next staged unit follows a barrier another mover's stores may hide behind */
+	for (uint32_t c = 0;; c++) {
+		const uint32_t sidx = c % kStages;
+		Stage &st = sh.stage[sidx];
+		mbar_wait(&sh.full[sidx], (c / kStages) & 1);
+		if (st.stop) break;
+		upfence = true;
+		const MoverFill f = {st, st.nseg, st.nunits, st.nwaves};
+		/* RAW/WAW/WAR against fill c-drain: before touching a flagged unit, wait until every mover has left that fill */
+		const uint32_t drain = st.drain;
+		bool drained = !(drain && c >= drain);
+		if (!drained && st.drain_upfront) {
+			wait_fill_moved(sh, c - drain);
+			drained = true;
+		}
+		/* shared kernels: units are drawn from a counter (mover 0 spends part of its time publishing) unless the fill
+		 * has waves, whose barrier wants every mover to walk the same list */
+		const bool dyn = kMoverReap && f.nw == 1;
+		for (uint32_t w = 0; w < f.nw; w++) {
+			for (uint32_t u = dyn ? next_unit(st, true, 0, lane) : (uint32_t)mw, u_next = 0; u < f.nunits; u = u_next) {
+				u_next = next_unit(st, dyn, u, lane);	/* drawn before this unit moves: the counter's latency hides behind the loads */
+				const Segment &g = f.seg_of(u);
+				if (f.nw > 1 && (g.wave & kSegWaveMask) != w) continue;
+				if ((g.wave & kSegWaitsForDrain) && !drained) {
+					wait_fill_moved(sh, c - drain);
+					drained = true;
+					upfence = true;
+				}
+				move_seg_unit<kMirrored, kStaged>(lun, f, g, u, u_next, w, drained, lane, sh.ustage[mw], sh.ubar[mw], us, upfence);
+			}
+			if (f.nw > 1) { movers_barrier(); upfence = true; }
+		}
+		if (mw == 0 && lane == 0 && st.lat_ntgt) tally_fill_latency(sh, st, lun);
+		__syncwarp();
+		if (lane == 0) mbar_arrive(&sh.empty[sidx]);
+		if constexpr (kMoverReap) {
+			if (mw == 0) {
+				/* every mover is done with the fill: publish its completions (in ring order across CTAs, reap_stage
+				 * waits for the fills before it) and hand the stage back to the parser */
+				wait_fill_moved(sh, c);
+				reap_stage(st, lane, &sh.pub_q, &sh.pub_end);
+				__syncwarp();
+				if (lane == 0) mbar_arrive(&sh.released[sidx]);
+			}
+		}
+	}
+}
+
+__device__ __forceinline__ void init_cta_shared(CtaShared &sh)
+{
+	for (int s = 0; s < kStages; s++) {
+		mbar_init(&sh.full[s], 1);
+		mbar_init(&sh.empty[s], kMovers);
+		mbar_init(&sh.released[s], 1);
+	}
+	mbar_init(&sh.req_bar[0], 1);
+	mbar_init(&sh.req_bar[1], 1);
+	for (int w = 0; w < kMovers; w++) { mbar_init(&sh.ubar[w][0], 1); mbar_init(&sh.ubar[w][1], 1); }
+	sh.pub_q = nullptr;
+	sh.pub_end = 0;
+	for (int t = 0; t < OIMGPU_CTRLR_MAX_DEVS; t++) sh.lat_ns[t][0] = sh.lat_ns[t][1] = sh.lat_ns[t][2] = 0;
+	asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+}
+
 /* kMoverReap: mover warp 0 publishes the completions of a fill instead of the parser.  Always so with shared queues
  * (§ QShare); also for launches that serve guest virtqueues only, where publishing means byte stores into 32 response
  * buffers, 32 used elements and a fence that waits for every load the parser has in flight - time taken from the
@@ -1259,67 +1656,20 @@ __device__ __forceinline__ uint32_t find_shared_work(const KickHeader *hdr, cons
 /* kStaged: byte-granular units go through this warp's staging buffer (move_unit_via_smem) - the kernel is launched
  * with the 29 KB the buffers take.  The mirror kernels (NVLink-bound, compact path) and the vring kernel do without:
  * the virtqueue parser lives on the L1 (descriptor tables, rings, the memory table), and two CTAs with staging
- * buffers leave it a third of the L1 they would have without (tools/exp_vq_variants.sh compares: shared memory that
- * nothing used costs the same), while guests' buffers are sector-aligned as a rule */
+ * buffers leave it a third of the L1 they would have without (measured: shared memory that nothing used costs the
+ * same), while guests' buffers are sector-aligned as a rule */
 template <bool kMirrored, bool kShared, bool kMoverReap = kShared, bool kStaged = !kMirrored>
 __device__ __forceinline__ void lun_queue_body(LunCtx *lun, KickHeader *hdr, const QueueDesc *queues)
 {
 	extern __shared__ __align__(16) unsigned char smem_raw[];
 	CtaShared &sh = *reinterpret_cast<CtaShared *>(smem_raw);
 	const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-
 	if (hdr->persistent && hdr->dispatcher && blockIdx.x == gridDim.x - 1) {
-		/* ======================= DISPATCHER (see KickHeader) ======================= */
-		if (warp != 0) return;
-		const uint32_t nq = hdr->nqueues;
-		uint64_t last_change = globaltimer_ns();
-		for (;;) {
-			bool changed = false;
-			for (uint32_t base = 0; base < nq; base += 32) {
-				const uint32_t qi = base + lane;
-				if (qi < nq) {
-					const QueueDesc &q = queues[qi];
-					const uint32_t v = q.mode == QMODE_VRING ? (uint32_t)ld_vol16(q.vq_avail + 2) : ld_vol32(q.doorbell);
-					if (v != ld_vol32(&q.vq_state->hint)) {
-						st_vol32(&q.vq_state->hint, v);
-						changed = true;
-					}
-				}
-			}
-			changed = __any_sync(0xffffffffu, changed);
-			uint32_t quit = 0;
-			if (lane == 0) {
-				const uint64_t now = globaltimer_ns();
-				if (changed) last_change = now;
-				quit = ld_vol32(hdr->stop) != 0;
-				if (!quit && hdr->idle_timeout_ms && now - last_change > (uint64_t)hdr->idle_timeout_ms * 1000000ull) quit = 1;
-				if (quit) st_vol32(&hdr->stop_mirror, 1u);
-			}
-			if (__shfl_sync(0xffffffffu, quit, 0)) break;
-		}
-		if (lane == 0) {
-			__threadfence_system();
-			atomicAdd_system(const_cast<uint32_t *>(hdr->exited), 1u);
-		}
+		if (warp == 0) dispatcher_cta(hdr, queues, lane);
 		return;
 	}
-
-	if (tid == 0) {
-		for (int s = 0; s < kStages; s++) {
-			mbar_init(&sh.full[s], 1);
-			mbar_init(&sh.empty[s], kMovers);
-			mbar_init(&sh.released[s], 1);
-		}
-		mbar_init(&sh.req_bar[0], 1);
-		mbar_init(&sh.req_bar[1], 1);
-		for (int w = 0; w < kMovers; w++) { mbar_init(&sh.ubar[w][0], 1); mbar_init(&sh.ubar[w][1], 1); }
-		sh.pub_q = nullptr;
-		sh.pub_end = 0;
-		for (int t = 0; t < OIMGPU_CTRLR_MAX_DEVS; t++) sh.lat_ns[t][0] = sh.lat_ns[t][1] = sh.lat_ns[t][2] = 0;
-		asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-	}
+	if (tid == 0) init_cta_shared(sh);
 	__syncthreads();
-
 	if (warp == 0) {
 		/* ======================= PARSER ======================= */
 		const LunCtx &L = *lun;
@@ -1333,9 +1683,7 @@ __device__ __forceinline__ void lun_queue_body(LunCtx *lun, KickHeader *hdr, con
 		uint32_t pass_no = 0;			/* passes parsed by this CTA: index into the hazard history ring */
 		if (lane < kStages) { sh.hist[lane].writers = 0; sh.hist[lane].touching = 0; }
 		__syncwarp();
-		uint32_t st_rd = 0, st_wr = 0, st_um = 0, st_er = 0;
-		uint32_t mix_r = 0, mix_w = 0;		/* good reads / writes + unmaps of ANY target: the session's mix */
-		unsigned long long st_rb = 0, st_wb = 0, st_ub = 0;
+		IoStats stats;
 		bool first = true;
 		/* Who publishes a fill's completions.  One CTA per queue: the parser, when it needs the stage again.
 		 * Shared queues: completions are published in ring order ACROSS CTAs, so a fill that waits for the
@@ -1602,79 +1950,10 @@ __device__ __forceinline__ void lun_queue_body(LunCtx *lun, KickHeader *hdr, con
 				const uint32_t haz = active ? s.hazard : 0;
 				const uint64_t lo = s.store_lo, hi = s.store_hi;
 
-				/* hazards against the passes whose movers may still be running (the stage ring only stops
-				 * the parser from refilling a stage; a mover may be two fills behind).  The segments of a
-				 * request that conflicts with one of them are flagged; a mover that reaches a flagged unit
-				 * first waits until the conflicting fill is finished, everything else in the pass proceeds
-				 * at once.  (Waiting for fill c-d's `empty` barrier covers all older ones too: a mover
-				 * arrives there only after finishing its share of every earlier fill.) */
-				uint32_t drain = 0;	/* 0 = none, d = fill c-d must be finished before flagged units move */
-				bool cross = false;	/* this lane's request is one of the conflicting ones */
-				const uint32_t writers = __ballot_sync(0xffffffffu, haz >= 2);
-				const uint32_t touching = __ballot_sync(0xffffffffu, haz != 0);
-				/* This pass's ranges and signatures go into a small ring in shared memory */
-				HazPass &cur = sh.hist[pass_no % kStages];
-				/* a read-only stream never needs signatures: while neither this pass nor the ones it could
-				 * be compared with contain a writer, the pass is left unsigned (= "dense": whoever meets
-				 * it later falls back to the exact ranges) */
-				bool sign = writers != 0;
-#pragma unroll
-				for (int h = 1; h <= kHist; h++) {
-					if ((uint32_t)h <= pass_no) sign |= sh.hist[(pass_no - h) % kStages].writers != 0;
-				}
-				if (sign) {
-					for (int k = lane; k < kSigWords; k += 32) { cur.sig_r[k] = 0; cur.sig_w[k] = 0; }
-				}
-				cur.lo[lane] = lo;
-				cur.hi[lane] = hi;
-				cur.haz[lane] = (uint8_t)haz;
-				if (lane == 0) { cur.writers = writers; cur.touching = touching; cur.dense = sign ? 0 : 1; }
-				__syncwarp();
-				const uint64_t g0 = lo >> 12, g1 = haz ? (hi - 1) >> 12 : g0;
-				const bool mydense = haz == 3 || (haz && g1 - g0 >= (uint64_t)kSigMaxGranules);
-				bool wcollide = false;	/* a writer found one of its granules already written in this pass */
-				if (!sign) { /* nothing to publish */ }
-				else if (mydense) cur.dense = 1;
-				else if (haz) {
-					for (uint64_t g = g0; g <= g1; g++) {
-						const uint32_t idx = sig_index(g);
-						if (haz >= 2) wcollide |= (atomicOr(&cur.sig_w[idx >> 5], 1u << (idx & 31)) >> (idx & 31)) & 1u;
-						else atomicOr(&cur.sig_r[idx >> 5], 1u << (idx & 31));
-					}
-				}
-				__syncwarp();
-				/* against the kStages-1 passes before this one: signature first, exact ranges only for the
-				 * requests the signature cannot clear */
-#pragma unroll
-				for (int h = kHist; h >= 1; h--) {
-					if ((uint32_t)h > pass_no) continue;
-					const HazPass &pp = sh.hist[(pass_no - h) % kStages];
-					const uint32_t candidates = haz >= 2 ? pp.touching : haz ? pp.writers : 0u;
-					bool maybe = false;
-					if (candidates) {
-						if (mydense || pp.dense) maybe = true;
-						else {
-							for (uint64_t g = g0; g <= g1; g++) {
-								const uint32_t idx = sig_index(g);
-								uint32_t word = pp.sig_w[idx >> 5];
-								if (haz >= 2) word |= pp.sig_r[idx >> 5];
-								maybe |= (word >> (idx & 31)) & 1u;
-							}
-						}
-					}
-					bool hit = false;
-					if (maybe) {
-						uint32_t scan = candidates;
-						while (scan) {
-							const int j = __ffs(scan) - 1;
-							scan &= scan - 1;
-							if (haz == 3 || pp.haz[j] == 3 || (lo < pp.hi[j] && pp.lo[j] < hi)) hit = true;
-						}
-					}
-					cross |= hit;
-					if (__any_sync(0xffffffffu, hit)) drain = (uint32_t)h;	/* nearest pass wins */
-				}
+				const PassHazards hz = cross_pass_hazards(sh.hist, pass_no, haz, lo, hi, lane);
+				const HazPass &cur = sh.hist[pass_no % kStages];
 				pass_no++;
+				const uint32_t writers = hz.writers; const uint32_t drain = hz.drain; const bool cross = hz.cross;
 
 				if (shared) {
 					/* Passes of other CTAs on this queue.  Parse results are published in ring order; with them
@@ -1745,73 +2024,11 @@ __device__ __forceinline__ void lun_queue_body(LunCtx *lun, KickHeader *hdr, con
 					}
 				}
 
-				/* hazards inside the pass -> waves.  Writers are visited in ring order; a writer is
-				 * pushed behind every earlier request it overlaps, every later overlapping request
-				 * behind the writer.  Most passes have no overlap at all: the signatures say so. */
-				uint16_t wave = 0;
-				uint32_t nwaves = 1;
-				bool inpass = false;
-				if (writers && (touching & (touching - 1)) && haz) {
-					if (mydense || cur.dense) inpass = true;
-					else if (haz >= 2) {
-						inpass = wcollide;
-						for (uint64_t g = g0; g <= g1; g++) {
-							const uint32_t idx = sig_index(g);
-							inpass |= (cur.sig_r[idx >> 5] >> (idx & 31)) & 1u;
-						}
-					} else {
-						for (uint64_t g = g0; g <= g1; g++) {
-							const uint32_t idx = sig_index(g);
-							inpass |= (cur.sig_w[idx >> 5] >> (idx & 31)) & 1u;
-						}
-					}
-				}
-				if (__any_sync(0xffffffffu, inpass)) {
-					uint32_t w = writers;
-					while (w) {
-						const int j = __ffs(w) - 1;
-						w &= w - 1;
-						const uint64_t jlo = __shfl_sync(0xffffffffu, lo, j);
-						const uint64_t jhi = __shfl_sync(0xffffffffu, hi, j);
-						const uint32_t jhaz = __shfl_sync(0xffffffffu, haz, j);
-						const bool overlap = haz != 0 && lane != j &&
-							(jhaz == 3 || haz == 3 || (lo < jhi && jlo < hi));
-						uint32_t need = (overlap && lane < j) ? (uint32_t)wave + 1 : 0;
-						need = __reduce_max_sync(0xffffffffu, need);
-						if (lane == j && need > wave) wave = (uint16_t)need;
-						const uint32_t jw = __shfl_sync(0xffffffffu, (uint32_t)wave, j);
-						if (overlap && lane > j && jw + 1 > wave) wave = (uint16_t)(jw + 1);
-					}
-					nwaves = __reduce_max_sync(0xffffffffu, (uint32_t)wave) + 1;
-				}
+				uint32_t nwaves;
+				const uint16_t wave = assign_waves(cur, hz, haz, lo, hi, lane, nwaves);
 
-				/* counters for get_bdevs_iostat */
 				const bool good = active && s.resp_valid && s.response == OIMGPU_S_OK && s.status == SC_GOOD;
-				const bool own = !good || s.tgt == L.target;	/* failures are booked on the session's device */
-				const bool ok = good && own;
-				st_rd += __popc(__ballot_sync(0xffffffffu, ok && s.op == OP_READ));
-				st_wr += __popc(__ballot_sync(0xffffffffu, ok && s.op == OP_WRITE));
-				/* UNMAP reaches the bdev once per applied descriptor, whatever the command's final status */
-				const bool um = active && s.resp_valid && s.response == OIMGPU_S_OK && s.op == OP_UNMAP && s.tgt == L.target;
-				st_um += __reduce_add_sync(0xffffffffu, um ? s.nseg : 0u);
-				if (um) st_ub += s.unmap_bytes;
-				st_er += __popc(__ballot_sync(0xffffffffu, active && !good));
-				mix_r += __popc(__ballot_sync(0xffffffffu, good && s.op == OP_READ));
-				mix_w += __popc(__ballot_sync(0xffffffffu, good && (s.op == OP_WRITE || s.op == OP_UNMAP)));
-				if (ok && s.op == OP_READ) st_rb += s.length;
-				if (ok && s.op == OP_WRITE) st_wb += s.length;
-				if (active && s.resp_valid && s.response == OIMGPU_S_OK && s.tgt != L.target &&
-				    ((good && (s.op == OP_READ || s.op == OP_WRITE)) || s.op == OP_UNMAP)) {
-					/* another device of the controller: book it there (rare path, plain atomics) */
-					LunCtx *P = L.peer[s.tgt];
-					if (s.op == OP_UNMAP) {
-						if (s.nseg) { atomicAdd(&P->stats[2], (unsigned long long)s.nseg); atomicAdd(&P->stats[6], (unsigned long long)s.unmap_bytes); }
-					} else {
-						const int k = s.op == OP_READ ? 0 : 1;
-						atomicAdd(&P->stats[k], 1ull);
-						atomicAdd(&P->stats[4 + k], (unsigned long long)s.length);
-					}
-				}
+				stats.count(L, s, active, good);
 
 				/* rounds: as many whole requests as fit in one stage's segment table */
 				uint32_t r0 = 0;
@@ -1875,18 +2092,9 @@ __device__ __forceinline__ void lun_queue_body(LunCtx *lun, KickHeader *hdr, con
 						st.nseg = tot_seg;
 						st.nunits = tot_unit;
 						st.nwaves = nwaves;
-#if OIM_SPLIT_FILLS_STREAM
-						/* later fills of a split pass: with conflicts INSIDE the pass (waves) they wait for the fill
-						 * before them, up front; without, only the requests that conflict with an earlier pass wait,
-						 * for the fill before (which covers every older one; c - drain itself may be more than a
-						 * stage ring behind by now) */
-						st.drain = (r0 > 0) ? ((nwaves > 1 || drain) ? 1 : 0) : drain;
-						st.drain_upfront = r0 > 0 && nwaves > 1;
-#else
 						/* later fills of a split pass simply wait for the fill before them, up front */
 						st.drain = (r0 > 0) ? 1 : drain;
 						st.drain_upfront = r0 > 0;
-#endif
 						st.stop = 0;
 						st.ncpl = r1 - r0;
 						st.cpl_ring = q.cpls;
@@ -1952,154 +2160,8 @@ __device__ __forceinline__ void lun_queue_body(LunCtx *lun, KickHeader *hdr, con
 			__threadfence_system();
 			atomicAdd_system(const_cast<uint32_t *>(hdr->exited), 1u);
 		}
-		/* flush counters: one atomic per counter per CTA */
-		for (int o = 16; o; o >>= 1) {
-			st_rb += __shfl_xor_sync(0xffffffffu, st_rb, o);
-			st_wb += __shfl_xor_sync(0xffffffffu, st_wb, o);
-			st_ub += __shfl_xor_sync(0xffffffffu, st_ub, o);
-		}
-		if (lane == 0 && st_ub) atomicAdd(&lun->stats[6], st_ub);
-		if (lane == 0) {
-			if (st_rd) { atomicAdd(&lun->stats[0], (unsigned long long)st_rd); atomicAdd(&lun->stats[4], st_rb); }
-			if (st_wr) { atomicAdd(&lun->stats[1], (unsigned long long)st_wr); atomicAdd(&lun->stats[5], st_wb); }
-			if (st_um) atomicAdd(&lun->stats[2], (unsigned long long)st_um);
-			if (st_er) atomicAdd(&lun->stats[7], (unsigned long long)st_er);
-			if (mix_r) atomicAdd(&lun->mix[0], (unsigned long long)mix_r);
-			if (mix_w) atomicAdd(&lun->mix[1], (unsigned long long)mix_w);
-			/* every fill is retired: mover warp 0 is done adding */
-			for (int t = 0; t < OIMGPU_CTRLR_MAX_DEVS; t++) {
-				LunCtx *T = (t == lun->target) ? lun : lun->peer[t];
-				for (int k = 0; k < 3 && T; k++) {
-					if (sh.lat_ns[t][k]) atomicAdd(&T->stats[8 + k], sh.lat_ns[t][k]);
-				}
-			}
-		}
-	} else {
-		/* ======================= MOVERS ======================= */
-		const int mw = warp - 1;
-		UStage us = {nullptr, 0};	/* this warp's staging buffer (move_unit_via_smem) */
-		bool upfence = true;		/* the next staged unit follows a barrier another mover's stores may hide behind */
-		for (uint32_t c = 0;; c++) {
-			const uint32_t sidx = c % kStages;
-			Stage &st = sh.stage[sidx];
-			mbar_wait(&sh.full[sidx], (c / kStages) & 1);
-			if (st.stop) break;
-			upfence = true;
-			const uint32_t nseg = st.nseg, nunits = st.nunits, nw = st.nwaves;
-			/* RAW/WAW/WAR against fill c-drain: before touching a flagged unit, wait until every mover has
-			 * left that fill (a mover arrives on `empty` only after finishing its share of all earlier
-			 * fills too) */
-			const uint32_t drain = st.drain;
-			bool drained = !(drain && c >= drain);
-			if (!drained && st.drain_upfront) {
-				const uint32_t p = c - drain;
-				mbar_wait(&sh.empty[p % kStages], (p / kStages) & 1);
-				drained = true;
-			}
-			/* shared kernels: units are drawn from a counter (mover 0 spends part of its time publishing) unless
-			 * the fill has waves, whose barrier wants every mover to walk the same list */
-			const bool dyn = kMoverReap && nw == 1;
-			auto next_unit = [&](uint32_t u) -> uint32_t {
-				if (!dyn) return u + kMovers;
-				uint32_t v = 0;
-				if (lane == 0) v = atomicAdd(&st.unit_ctr, 1u);
-				return __shfl_sync(0xffffffffu, v, 0);
-			};
-			auto find_seg = [&](uint32_t u) -> uint32_t {
-				uint32_t lo = u, hi = nseg;	/* last segment with first_unit <= u */
-				/* as many units as segments: segment u IS unit u.  Taken for passes of small requests (the
-				 * 4 KiB case); long SG lists of single pages keep the search - the lookup's latency
-				 * spreads the movers' loads there */
-				if (nunits != nseg || nseg > (uint32_t)kPass) {
-					lo = 0;
-					while (hi - lo > 1) {
-						const uint32_t mid = (lo + hi) >> 1;
-						if (st.seg[mid].first_unit <= u) lo = mid; else hi = mid;
-					}
-				}
-				return lo;
-			};
-			for (uint32_t w = 0; w < nw; w++) {
-				for (uint32_t u = dyn ? next_unit(0) : (uint32_t)mw, u_next = 0; u < nunits; u = u_next) {
-					u_next = next_unit(u);	/* drawn before this unit moves: the counter's latency hides behind the loads */
-					const Segment &g = st.seg[find_seg(u)];
-					if (nw > 1 && (g.wave & kSegWaveMask) != w) continue;
-					if ((g.wave & kSegWaitsForDrain) && !drained) {
-						const uint32_t p = c - drain;
-						mbar_wait(&sh.empty[p % kStages], (p / kStages) & 1);
-						drained = true;
-						upfence = true;
-					}
-					const uint64_t off = (uint64_t)(u - g.first_unit) * kUnitBytes;
-					const uint32_t nbytes = (uint32_t)min((uint64_t)kUnitBytes, g.len - off);
-					const uint8_t *src = g.src;
-					uint8_t *dst = g.dst;
-					if (!kMirrored || !g.mirror) {
-						if constexpr (kMirrored) {
-							if (src) move_unit<true>(dst + off, src + off, nbytes, lane);
-							else zero_unit(dst + off, nbytes, lane);
-						} else {
-							if (!src) {
-								zero_unit(dst + off, nbytes, lane);
-							} else if ((((uintptr_t)(dst + off) | (uintptr_t)(src + off) | nbytes) & 15) == 0) {
-								move_unit(dst + off, src + off, nbytes, lane);
-							} else if constexpr (!kStaged || !OIM_USTAGE) {
-								move_unit(dst + off, src + off, nbytes, lane);
-							} else {
-								/* the unit this warp moves next, when it is known and nothing has to be waited for
-								 * before it may be read: its bytes are requested while this one is realigned */
-								uint8_t *ndst = nullptr; const uint8_t *nsrc = nullptr; uint32_t nn = 0;
-#if OIM_USTAGE_PREFETCH
-								if (u_next < nunits) {
-									const Segment &g2 = st.seg[find_seg(u_next)];
-									if (g2.src && (nw == 1 || (g2.wave & kSegWaveMask) == w) && (!(g2.wave & kSegWaitsForDrain) || drained)) {
-										const uint64_t off2 = (uint64_t)(u_next - g2.first_unit) * kUnitBytes;
-										nn = (uint32_t)min((uint64_t)kUnitBytes, g2.len - off2);
-										if ((((uintptr_t)(g2.dst + off2) | (uintptr_t)(g2.src + off2) | nn) & 15) != 0) { ndst = g2.dst + off2; nsrc = g2.src + off2; }
-									}
-								}
-#endif
-								move_unit_via_smem(dst + off, src + off, nbytes, lane, sh.ustage[mw], sh.ubar[mw], us, upfence, ndst, nsrc, nn);
-							}
-						}
-					} else {
-						const LunCtx &T = (g.mirror - 1 == lun->target) ? *lun : *lun->peer[g.mirror - 1];
-						mirror_unit(T, dst, src, off, nbytes, lane, T.nreplicas);
-					}
-				}
-				if (nw > 1) { movers_barrier(); upfence = true; }
-			}
-			if (mw == 0 && lane == 0 && st.lat_ntgt) {
-				const unsigned long long dt = globaltimer_ns() - st.t0;
-				for (uint32_t i = 0; i < st.lat_ntgt; i++) {
-					const uint32_t t = st.lat_tgt[i] & (OIMGPU_CTRLR_MAX_DEVS - 1);
-					unsigned long long *acc = sh.lat_ns[t];
-					acc[0] += dt * st.lat_n[i][0]; acc[1] += dt * st.lat_n[i][1]; acc[2] += dt * st.lat_n[i][2];
-					/* spdk_histogram_data_tally (histogram_data.h:120-160) of the fill's latency, once per request */
-					const LunCtx *T = (t == lun->target) ? lun : lun->peer[t];
-					unsigned long long *hist = T ? *reinterpret_cast<unsigned long long *const volatile *>(&T->hist) : nullptr;
-					if (hist && dt) {
-						const uint32_t clz = (uint32_t)__clzll((long long)dt);
-						const uint32_t range = clz <= 57u ? 57u - clz : 0u;
-						const uint32_t index = (uint32_t)(dt >> (range ? range - 1 : 0)) & 127u;
-						atomicAdd(&hist[(range << 7) + index], (unsigned long long)(st.lat_n[i][0] + st.lat_n[i][1] + st.lat_n[i][2]));
-					}
-				}
-			}
-			__syncwarp();
-			if (lane == 0) mbar_arrive(&sh.empty[sidx]);
-			if constexpr (kMoverReap) {
-				if (mw == 0) {
-					/* every mover is done with the fill: publish its completions (in ring order across CTAs,
-					 * reap_stage waits for the fills before it) and hand the stage back to the parser */
-					mbar_wait(&sh.empty[sidx], (c / kStages) & 1);
-					reap_stage(st, lane, &sh.pub_q, &sh.pub_end);
-					__syncwarp();
-					if (lane == 0) mbar_arrive(&sh.released[sidx]);
-				}
-			}
-		}
-	}
+		stats.flush(lun, sh, lane);
+	} else mover_warp<kMirrored, kMoverReap, kStaged>(sh, lun, warp - 1, lane);
 }
 
 /* the plain kernel carries no mirror code at all (a call in the mover loop would spill the
@@ -2188,7 +2250,43 @@ oim_digest_kernel(const uint64_t *p, uint64_t nwords, unsigned long long *out)
 	if ((threadIdx.x & 31) == 0) { atomicAdd(&out[0], a); atomicAdd(&out[1], b); }
 }
 
-/* staged: with the movers' staging buffers (the last member), for the kernels instantiated with kStaged */
-size_t lun_kernel_smem_bytes(bool staged) { return staged && OIM_USTAGE ? sizeof(CtaShared) : offsetof(CtaShared, ustage); }
+/* ---- host side: the five instantiations and what each is launched with ------------------------------------- */
+
+/* the kStaged instantiations carry the movers' staging buffers (the last member of CtaShared); the others keep the L1 */
+static size_t lun_kernel_smem_bytes(LunKernel k)
+{
+	const bool staged = k == LUN_KERNEL_QUEUE || k == LUN_KERNEL_SHARED_QUEUE;
+	return staged ? sizeof(CtaShared) : offsetof(CtaShared, ustage);
+}
+
+cudaError_t lun_kernels_init(int *ctas_per_sm)
+{
+	/* more than the 48 KB a kernel gets without asking */
+	cudaError_t e = cudaSuccess;
+	auto set_smem = [&](auto kernel, LunKernel k) {
+		if (e == cudaSuccess) e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lun_kernel_smem_bytes(k));
+	};
+	set_smem(oim_lun_queue_kernel, LUN_KERNEL_QUEUE);
+	set_smem(oim_lun_queue_mirror_kernel, LUN_KERNEL_QUEUE_MIRROR);
+	set_smem(oim_lun_vring_kernel, LUN_KERNEL_VRING);
+	set_smem(oim_lun_shared_queue_kernel, LUN_KERNEL_SHARED_QUEUE);
+	set_smem(oim_lun_shared_queue_mirror_kernel, LUN_KERNEL_SHARED_QUEUE_MIRROR);
+	if (e != cudaSuccess) return e;
+	return cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, oim_lun_queue_kernel, kThreads,
+							     lun_kernel_smem_bytes(LUN_KERNEL_QUEUE));
+}
+
+void launch_lun_kernel(LunKernel k, uint32_t grid, cudaStream_t stream, LunCtx *ctx, KickHeader *hdr, const QueueDesc *desc)
+{
+	const size_t smem = lun_kernel_smem_bytes(k);
+	switch (k) {
+	case LUN_KERNEL_QUEUE: oim_lun_queue_kernel<<<grid, kThreads, smem, stream>>>(ctx, hdr, desc); break;
+	case LUN_KERNEL_QUEUE_MIRROR: oim_lun_queue_mirror_kernel<<<grid, kThreads, smem, stream>>>(ctx, hdr, desc); break;
+	case LUN_KERNEL_VRING: oim_lun_vring_kernel<<<grid, kThreads, smem, stream>>>(ctx, hdr, desc); break;
+	case LUN_KERNEL_SHARED_QUEUE: oim_lun_shared_queue_kernel<<<grid, kThreads, smem, stream>>>(ctx, hdr, desc); break;
+	case LUN_KERNEL_SHARED_QUEUE_MIRROR: oim_lun_shared_queue_mirror_kernel<<<grid, kThreads, smem, stream>>>(ctx, hdr, desc); break;
+	default: break;
+	}
+}
 
 }  // namespace oimgpu

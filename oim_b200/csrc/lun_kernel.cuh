@@ -48,17 +48,8 @@ constexpr int kPass = OIMGPU_REQS_PER_PASS;	/* 32 = one warp of parser lanes */
 constexpr int kMovers = OIM_MOVERS;		/* mover warps per CTA */
 constexpr int kThreads = (1 + kMovers) * 32;	/* parser warp + movers */
 constexpr int kStages = OIM_STAGES;		/* parser -> mover pipeline depth */
-#ifndef OIM_USTAGE
-#define OIM_USTAGE 1		/* tuning builds: 0 = byte-granular units take the register path (move_unit_unaligned) */
-#endif
 #ifndef OIM_FILL_UNITS
 #define OIM_FILL_UNITS 256
-#endif
-#ifndef OIM_SPLIT_FILLS_STREAM
-#define OIM_SPLIT_FILLS_STREAM 0	/* tuning builds: 1 = later fills of a hazard-free split pass do not wait for the fill
-					 * before them (compare with tools/exp_fill_variants.sh before changing the
-					 * default): the wait re-aligns the seven movers every 256 units,
-					 * and movers that drift apart cost more than the bubble at the fill boundary */
 #endif
 constexpr int kFillUnits = OIM_FILL_UNITS;	/* units per stage fill (a request larger than that has a fill of its own) */
 constexpr int kSegCap = 256;			/* SG segments per stage (>= 256 UNMAP descriptors, >= 129 iovecs) */
@@ -296,18 +287,22 @@ struct __align__(16) CtaShared {
 	unsigned long long lat_ns[OIMGPU_CTRLR_MAX_DEVS][3];	/* mover warp 0, lane 0: summed latencies of this CTA per target (reads, writes, unmaps) */
 	/* one staging buffer per mover warp for units that are not 16-byte aligned on both sides: the aligned bytes
 	 * covering a unit (<= kUnitBytes + 16) land here by bulk copy and are realigned on the way out */
-#ifdef OIM_SMEM_PAD	/* tuning builds: shared memory that nothing uses (what does the smaller L1 cost?) */
-	uint8_t pad_[OIM_SMEM_PAD];
-#endif
 	/* LAST member: kernels without the staged path are launched without it (lun_kernel_smem_bytes) */
 	__align__(128) uint8_t ustage[kMovers][kUnitBytes + 128];
 };
-#ifndef OIM_SMEM_PATH_INLINE
-#define OIM_SMEM_PATH_INLINE __forceinline__
-#endif
-#ifndef OIM_USTAGE_PREFETCH
-#define OIM_USTAGE_PREFETCH 1	/* tuning builds: 0 = a staged unit is requested only when its turn has come */
-#endif
+
+/* the queue kernel's instantiations (lun_kernel.cu); the host picks one per launch */
+enum LunKernel : int {
+	LUN_KERNEL_QUEUE,		/* one CTA per queue */
+	LUN_KERNEL_QUEUE_MIRROR,	/* ... with mirrored bdevs */
+	LUN_KERNEL_VRING,		/* ... guest virtqueues only */
+	LUN_KERNEL_SHARED_QUEUE,	/* CTAs share the queues a pass at a time (KickHeader::shared) */
+	LUN_KERNEL_SHARED_QUEUE_MIRROR,
+	LUN_KERNEL_COUNT
+};
+/* gives every instantiation the shared memory it is launched with; *ctas_per_sm = occupancy of the queue kernels */
+cudaError_t lun_kernels_init(int *ctas_per_sm);
+void launch_lun_kernel(LunKernel k, uint32_t grid, cudaStream_t stream, LunCtx *ctx, KickHeader *hdr, const QueueDesc *desc);
 
 /* ------------------------------------------------------------------------------------------ */
 

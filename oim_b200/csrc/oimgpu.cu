@@ -29,14 +29,8 @@
 #include "lun_kernel.cuh"
 
 namespace oimgpu {
-__global__ void oim_lun_queue_kernel(LunCtx *lun, KickHeader *hdr, const QueueDesc *queues);
-__global__ void oim_lun_queue_mirror_kernel(LunCtx *lun, KickHeader *hdr, const QueueDesc *queues);
-__global__ void oim_lun_shared_queue_kernel(LunCtx *lun, KickHeader *hdr, const QueueDesc *queues);
-__global__ void oim_lun_vring_kernel(LunCtx *lun, KickHeader *hdr, const QueueDesc *queues);
-__global__ void oim_lun_shared_queue_mirror_kernel(LunCtx *lun, KickHeader *hdr, const QueueDesc *queues);
 __global__ void oim_copy_kernel(uint8_t *dst, const uint8_t *src, uint64_t nbytes);
 __global__ void oim_fill_kernel(uint8_t *dst, uint8_t fill, uint64_t nbytes);
-size_t lun_kernel_smem_bytes(bool staged);
 }  // namespace oimgpu
 
 using namespace oimgpu;
@@ -1378,14 +1372,8 @@ static int lun_open_on(const char *ctrlr, int scsi_target_num, int on_device, ui
 	CU_OK(cudaMalloc((void **)&L->d_vq_state, sizeof(VqState) * num_queues));
 	CU_OK(cudaMemsetAsync(L->d_vq_state, 0, sizeof(VqState) * num_queues, L->stream));
 	CU_OK(cudaStreamSynchronize(L->stream));
-	/* more than the 48 KB a kernel gets without asking */
-	CU_OK(cudaFuncSetAttribute(oim_lun_queue_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lun_kernel_smem_bytes(true)));
-	CU_OK(cudaFuncSetAttribute(oim_lun_queue_mirror_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lun_kernel_smem_bytes(false)));
-	CU_OK(cudaFuncSetAttribute(oim_lun_shared_queue_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lun_kernel_smem_bytes(true)));
-	CU_OK(cudaFuncSetAttribute(oim_lun_vring_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lun_kernel_smem_bytes(false)));
-	CU_OK(cudaFuncSetAttribute(oim_lun_shared_queue_mirror_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lun_kernel_smem_bytes(false)));
 	int per_sm = 0;
-	CU_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, oim_lun_queue_kernel, kThreads, lun_kernel_smem_bytes(true)));
+	CU_OK(lun_kernels_init(&per_sm));
 	if (per_sm < 1) per_sm = 1;
 	L->grid_cap = L->sm_count * per_sm;
 	int rc = refresh_peers_locked(L.get());
@@ -1528,19 +1516,72 @@ static uint32_t share_max_queues(const oimgpu_lun *L)
 	return (uint32_t)L->grid_cap * 160 / 296;
 }
 
-static void launch_lun_kernel(oimgpu_lun *L, uint32_t grid, bool shared, bool vrings_only = false)
+static void launch_queue_kernel(oimgpu_lun *L, uint32_t grid, bool shared, bool vrings_only)
 {
-	/* the kernels with the staged byte-granular path carry the movers' staging buffers; the others keep the L1 */
-	const size_t smem = lun_kernel_smem_bytes(true), lean = lun_kernel_smem_bytes(false);
-	KickHeader *kh = (KickHeader *)L->d_kick;
-	if (!shared && !L->any_mirror && vrings_only && !getenv("OIMGPU_NO_VRING_KERNEL")) {
-		oim_lun_vring_kernel<<<grid, kThreads, lean, L->stream>>>(L->d_ctx, kh, L->d_desc);
-		return;
-	}
-	if (shared && L->any_mirror) oim_lun_shared_queue_mirror_kernel<<<grid, kThreads, lean, L->stream>>>(L->d_ctx, kh, L->d_desc);
-	else if (shared) oim_lun_shared_queue_kernel<<<grid, kThreads, smem, L->stream>>>(L->d_ctx, kh, L->d_desc);
-	else if (L->any_mirror) oim_lun_queue_mirror_kernel<<<grid, kThreads, lean, L->stream>>>(L->d_ctx, kh, L->d_desc);
-	else oim_lun_queue_kernel<<<grid, kThreads, smem, L->stream>>>(L->d_ctx, kh, L->d_desc);
+	LunKernel k;
+	if (!shared && !L->any_mirror && vrings_only && !getenv("OIMGPU_NO_VRING_KERNEL")) k = LUN_KERNEL_VRING;
+	else if (shared) k = L->any_mirror ? LUN_KERNEL_SHARED_QUEUE_MIRROR : LUN_KERNEL_SHARED_QUEUE;
+	else k = L->any_mirror ? LUN_KERNEL_QUEUE_MIRROR : LUN_KERNEL_QUEUE;
+	launch_lun_kernel(k, grid, L->stream, L->d_ctx, (KickHeader *)L->d_kick, L->d_desc);
+}
+
+/* ---- the QueueDesc records of a launch, one builder per kind of queue ---- */
+
+/* caller-owned device arrays, served once from slot 0 */
+static QueueDesc desc_device_arrays(oimgpu_lun *L, uint32_t q)
+{
+	const Queue &Q = L->queues[q];
+	QueueDesc D;
+	memset(&D, 0, sizeof(D));
+	D.vq_state = L->d_vq_state + q;
+	D.reqs = Q.dev_reqs;
+	D.iovs = Q.dev_iovs;
+	D.cpls = Q.dev_cpls ? Q.dev_cpls : Q.d_cpls;
+	D.ring_mask = 0xffffffffu;
+	D.iov_mask = 0xffffffffu;
+	D.iov_limit = Q.dev_iov_limit;
+	D.head = 0;
+	D.count = Q.dev_count;
+	return D;
+}
+
+/* the library's slot ring (the caller sets head / count, or the poller's doorbells) */
+static QueueDesc desc_slot_ring(oimgpu_lun *L, uint32_t q)
+{
+	const Queue &Q = L->queues[q];
+	QueueDesc D;
+	memset(&D, 0, sizeof(D));
+	D.vq_state = L->d_vq_state + q;
+	D.reqs = Q.d_reqs;
+	D.iovs = Q.d_iovs;
+	D.cpls = Q.d_cpls;
+	D.ring_mask = L->queue_size - 1;
+	D.iov_mask = L->iov_cap - 1;
+	return D;
+}
+
+/* an attached guest virtqueue; the parser lanes build their SG rows in d_iov_scratch */
+static QueueDesc desc_virtqueue(oimgpu_lun *L, uint32_t q)
+{
+	const Queue &Q = L->queues[q];
+	QueueDesc D;
+	memset(&D, 0, sizeof(D));
+	D.mode = QMODE_VRING;
+	D.iovs = L->d_iov_scratch;
+	D.vq_size = Q.vq_size;
+	D.vq_desc = Q.vq_desc;
+	D.vq_avail = Q.vq_avail;
+	D.vq_used = Q.vq_used;
+	D.vq_in_hbm = Q.vq_in_hbm ? 1 : 0;
+	D.vq_state = L->d_vq_state + q;
+	return D;
+}
+
+/* [grid_cap][32][kIovRow] SG rows for the parser lanes of virtqueue mode */
+static cudaError_t ensure_iov_scratch(oimgpu_lun *L)
+{
+	if (L->d_iov_scratch) return cudaSuccess;
+	return cudaMalloc((void **)&L->d_iov_scratch, sizeof(oimgpu_iov) * (size_t)L->grid_cap * kPass * kIovRow);
 }
 
 extern "C" int oimgpu_kick(oimgpu_lun *L)
@@ -1572,44 +1613,19 @@ extern "C" int oimgpu_kick(oimgpu_lun *L)
 		Queue &Q = L->queues[q];
 		if (Q.dev_count) {
 			passes += (Q.dev_count + kPass - 1) / kPass;
-			QueueDesc &D = h_desc[nd++];
-			memset(&D, 0, sizeof(D));
-			D.vq_state = L->d_vq_state + q;
-			D.reqs = Q.dev_reqs;
-			D.iovs = Q.dev_iovs;
-			D.cpls = Q.dev_cpls ? Q.dev_cpls : Q.d_cpls;
-			D.ring_mask = 0xffffffffu;
-			D.iov_mask = 0xffffffffu;
-			D.iov_limit = Q.dev_iov_limit;
-			D.head = 0;
-			D.count = Q.dev_count;
+			h_desc[nd++] = desc_device_arrays(L, q);
 			Q.dev_count = 0;
 		}
 		if (Q.vq_pending) {
 			passes += (Q.vq_size + kPass - 1) / kPass;
 			nvring++;
-			QueueDesc &D = h_desc[nd++];
-			memset(&D, 0, sizeof(D));
-			D.mode = QMODE_VRING;
-			D.iovs = L->d_iov_scratch;
-			D.vq_size = Q.vq_size;
-			D.vq_desc = Q.vq_desc;
-			D.vq_avail = Q.vq_avail;
-			D.vq_used = Q.vq_used;
-			D.vq_in_hbm = Q.vq_in_hbm ? 1 : 0;
-			D.vq_state = L->d_vq_state + q;
+			h_desc[nd++] = desc_virtqueue(L, q);
 			Q.vq_pending = false;
 		}
 		if (Q.tail != Q.kicked) {
 			passes += (Q.tail - Q.kicked + kPass - 1) / kPass;
 			QueueDesc &D = h_desc[nd++];
-			memset(&D, 0, sizeof(D));
-			D.vq_state = L->d_vq_state + q;
-			D.reqs = Q.d_reqs;
-			D.iovs = Q.d_iovs;
-			D.cpls = Q.d_cpls;
-			D.ring_mask = L->queue_size - 1;
-			D.iov_mask = L->iov_cap - 1;
+			D = desc_slot_ring(L, q);
 			D.head = Q.kicked;
 			D.count = Q.tail - Q.kicked;
 			Q.kicked = Q.tail;
@@ -1648,7 +1664,7 @@ extern "C" int oimgpu_kick(oimgpu_lun *L)
 	CU_OK(cudaMemcpyAsync(L->d_kick, L->h_kick[slot], sizeof(KickHeader) + sizeof(QueueDesc) * nd, cudaMemcpyHostToDevice, L->stream));
 	CU_OK(cudaEventRecord(L->kick_ev[slot], L->stream));
 	L->kicks++;
-	launch_lun_kernel(L, grid, shared, nvring == nd);
+	launch_queue_kernel(L, grid, shared, nvring == nd);
 	CU_OK(cudaGetLastError());
 	CU_OK(cudaMemcpyAsync((void *)L->h_mix, (const uint8_t *)L->d_ctx + offsetof(LunCtx, mix), sizeof(unsigned long long) * 2,
 			      cudaMemcpyDeviceToHost, L->stream));
@@ -2111,10 +2127,8 @@ extern "C" int oimgpu_vq_attach(oimgpu_lun *L, uint32_t q, const void *desc, con
 	if (L->poller_active) return -EBUSY;
 	CU_OK(cudaSetDevice(L->device));
 	CU_OK(cudaStreamSynchronize(L->stream));
-	if (!L->d_iov_scratch) {
-		CU_OK(cudaMalloc((void **)&L->d_iov_scratch, sizeof(oimgpu_iov) * (size_t)L->grid_cap * kPass * kIovRow));
-	}
-	VqState st = { last_avail_idx, last_used_idx, last_avail_idx, 0 };
+	CU_OK(ensure_iov_scratch(L));
+	VqState st ={ last_avail_idx, last_used_idx, last_avail_idx, 0 };
 	CU_OK(h2d_sync(L, L->d_vq_state + q, &st, sizeof(st)));
 	Queue &Q = L->queues[q];
 	Q.vq_desc = (const uint8_t *)desc;
@@ -2176,9 +2190,7 @@ extern "C" int oimgpu_lun_start_poller(oimgpu_lun *L, uint32_t max_ctas, uint32_
 	if (L->poller_active) return -EALREADY;
 	CU_OK(cudaSetDevice(L->device));
 	CU_OK(cudaStreamSynchronize(L->stream));
-	if (!L->d_iov_scratch) {
-		CU_OK(cudaMalloc((void **)&L->d_iov_scratch, sizeof(oimgpu_iov) * (size_t)L->grid_cap * kPass * kIovRow));
-	}
+	CU_OK(ensure_iov_scratch(L));
 	const int slot = (int)(L->kicks % oimgpu_lun::kKickSlots);
 	QueueDesc *h_desc = (QueueDesc *)(L->h_kick[slot] + sizeof(KickHeader));
 	uint32_t nd = 0;
@@ -2189,27 +2201,12 @@ extern "C" int oimgpu_lun_start_poller(oimgpu_lun *L, uint32_t max_ctas, uint32_
 		Queue &Q = L->queues[q];
 		if (Q.dev_count || Q.tail != Q.kicked) return -EBUSY;	/* drain pending launches first */
 		if (Q.vq_size) {
-			QueueDesc &D = h_desc[nd++];
-			memset(&D, 0, sizeof(D));
-			D.mode = QMODE_VRING;
-			D.iovs = L->d_iov_scratch;
-			D.vq_size = Q.vq_size;
-			D.vq_desc = Q.vq_desc;
-			D.vq_avail = Q.vq_avail;
-			D.vq_used = Q.vq_used;
-			D.vq_in_hbm = Q.vq_in_hbm ? 1 : 0;
-			D.vq_state = L->d_vq_state + q;
+			h_desc[nd++] = desc_virtqueue(L, q);
 		} else {
 			QueueDesc &D = h_desc[nd++];
-			memset(&D, 0, sizeof(D));
-			D.reqs = Q.d_reqs;
-			D.iovs = Q.d_iovs;
-			D.cpls = Q.d_cpls;
-			D.ring_mask = L->queue_size - 1;
-			D.iov_mask = L->iov_cap - 1;
+			D = desc_slot_ring(L, q);
 			D.doorbell = &L->d_door[q].tail;
 			D.done = &L->d_door[q].done;
-			D.vq_state = L->d_vq_state + q;
 			/* everything kicked so far was served by launches: the poller starts from there */
 			L->h_door[q].tail = Q.kicked;
 			L->h_door[q].done = Q.kicked;
@@ -2261,7 +2258,7 @@ extern "C" int oimgpu_lun_start_poller(oimgpu_lun *L, uint32_t max_ctas, uint32_
 	{
 		uint32_t nv = 0;
 		for (uint32_t q = 0; q < L->num_queues; q++) nv += L->queues[q].vq_size != 0;
-		launch_lun_kernel(L, grid + 1, shared, nv == nd);
+		launch_queue_kernel(L, grid + 1, shared, nv == nd);
 	}
 	if (shared) L->shared_launches++;
 	CU_OK(cudaGetLastError());

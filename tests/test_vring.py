@@ -6,7 +6,7 @@ import pytest
 import util
 from oim_b200 import traces, vring
 
-# the kernels that serve a virtqueue-only kick, and the environment that selects each (liboimgpu.so launch_lun_kernel)
+# the kernels that serve a virtqueue-only kick, and the environment that selects each (liboimgpu.so launch_queue_kernel)
 VQ_KERNELS = {
     "shared": {"OIMGPU_NO_SHARED_QUEUES": None, "OIMGPU_SHARE_MAX_QUEUES": None, "OIMGPU_NO_VRING_KERNEL": None},
     # oim_lun_vring_kernel: one CTA per queue, the register realign path (move_unit_unaligned)

@@ -58,7 +58,7 @@ def environ(**kv: str | None):
         put(old)
 
 
-# The queue-kernel variants a single-queue trace can be pinned to (liboimgpu.so launch_lun_kernel):
+# The queue-kernel variants a single-queue trace can be pinned to (liboimgpu.so launch_queue_kernel):
 #   shared         oim_lun_shared_queue_kernel         the CTAs take the queue a pass at a time
 #   exclusive      oim_lun_queue_kernel                one CTA owns the queue (OIMGPU_NO_SHARED_QUEUES=1)
 #   mirror         oim_lun_queue_mirror_kernel         two replicas on cuda:0, one CTA per queue
