@@ -1,0 +1,204 @@
+/*
+ * copy_chan.cu - host memory for the GPU (registration, on-demand pinning) and the asynchronous copy channel.
+ */
+#include <deque>
+
+#include "host_state.h"
+
+extern "C" int oimgpu_mem_register(void *addr, size_t len)
+{
+	std::lock_guard<std::mutex> lk(g.mu);
+	if (!g.inited) return -ENODEV;
+	if (!addr || !len) return -EINVAL;
+	cudaError_t e = cudaHostRegister(addr, len, cudaHostRegisterMapped | cudaHostRegisterPortable);
+	if (e != cudaSuccess) {
+		(void)cudaGetLastError();
+		return e == cudaErrorHostMemoryAlreadyRegistered ? -EEXIST : -EFAULT;
+	}
+	g.registered[addr] = len;
+	return 0;
+}
+
+/* the address the GPU uses for a byte of registered host memory (identical to the host address on
+ * systems with a unified address space for registered memory, but that is the driver's call) */
+extern "C" int oimgpu_mem_device_addr(const void *addr, uint64_t *dev)
+{
+	if (!addr || !dev) return -EINVAL;
+	if (!g.inited || g.control_only) return -ENODEV;
+	void *d = nullptr;
+	cudaError_t e = cudaHostGetDevicePointer(&d, const_cast<void *>(addr), 0);
+	if (e != cudaSuccess) {
+		(void)cudaGetLastError();
+		return -EFAULT;
+	}
+	*dev = (uint64_t)(uintptr_t)d;
+	return 0;
+}
+
+extern "C" int oimgpu_mem_unregister(void *addr)
+{
+	std::lock_guard<std::mutex> lk(g.mu);
+	auto it = g.registered.find(addr);
+	if (it == g.registered.end()) return -ENOENT;
+	/* cuMemHostUnregister waits for the GPUs to go idle while holding a driver lock that every launch
+	 * needs: with a resident poller anywhere that is a deadlock, not a delay (seen: one VM's teardown
+	 * against another VM's poller restart).  Same remedy as for cudaFree. */
+	{
+		ParkedPollers parked(-1);
+		cudaHostUnregister(addr);
+	}
+	g.registered.erase(it);
+	return 0;
+}
+
+/* ---- asynchronous copy channel (the engine behind integration/spdk/copy_engine_oimgpu.c) ------------- */
+
+namespace {
+std::mutex g_pin_mu;
+std::map<uintptr_t, uintptr_t> g_pinned;	/* [start, end) of host ranges pinned by oimgpu_mem_ensure, disjoint */
+}
+
+void oimgpu::unpin_all_host_ranges()
+{
+	std::lock_guard<std::mutex> lk(g_pin_mu);
+	for (auto &kv : g_pinned) {
+		if (cudaHostUnregister((void *)kv.first) != cudaSuccess) (void)cudaGetLastError();
+	}
+	g_pinned.clear();
+}
+
+static bool pin_range(uintptr_t a, uintptr_t b)
+{
+	cudaError_t e = cudaHostRegister((void *)a, b - a, cudaHostRegisterMapped | cudaHostRegisterPortable);
+	if (e == cudaSuccess) return true;
+	(void)cudaGetLastError();
+	return e == cudaErrorHostMemoryAlreadyRegistered;	/* by someone else (cudaHostAlloc, oimgpu_mem_register): fine */
+}
+
+extern "C" int oimgpu_mem_ensure(const void *addr, size_t len)
+{
+	if (!g.inited || g.control_only) return -ENODEV;
+	if (!addr || !len) return 0;
+	cudaPointerAttributes attr{};
+	if (cudaPointerGetAttributes(&attr, addr) == cudaSuccess && attr.type != cudaMemoryTypeUnregistered) {
+		/* device memory, or host memory CUDA already knows: check the far end too (a range may straddle) */
+		cudaPointerAttributes last{};
+		if (cudaPointerGetAttributes(&last, (const uint8_t *)addr + len - 1) == cudaSuccess && last.type != cudaMemoryTypeUnregistered) return 0;
+	}
+	(void)cudaGetLastError();
+	const uintptr_t page = 4096, big = 2u << 20;
+	uintptr_t a = (uintptr_t)addr & ~(page - 1), b = ((uintptr_t)addr + len + page - 1) & ~(page - 1);
+	std::lock_guard<std::mutex> lk(g_pin_mu);
+	/* walk the gaps between what is already pinned */
+	while (a < b) {
+		auto it = g_pinned.upper_bound(a);
+		if (it != g_pinned.begin()) {
+			auto pv = std::prev(it);
+			if (pv->second > a) { a = pv->second; continue; }	/* inside a pinned range: skip it */
+		}
+		uintptr_t gap_end = (it != g_pinned.end() && it->first < b) ? it->first : b;
+		/* try the whole 2 MiB-aligned surroundings first (a big buffer then takes few registrations), clipped to
+		 * the neighbours; fall back to exactly the pages asked for (the surroundings may not be mapped) */
+		uintptr_t lo = a & ~(big - 1), hi = (gap_end + big - 1) & ~(big - 1);
+		if (it != g_pinned.begin() && std::prev(it)->second > lo) lo = std::prev(it)->second;
+		if (it != g_pinned.end() && it->first < hi) hi = it->first;
+		if (!(lo == a && hi == gap_end) && pin_range(lo, hi)) {
+			g_pinned[lo] = hi;
+		} else if (pin_range(a, gap_end)) {
+			g_pinned[a] = gap_end;
+			lo = a; hi = gap_end;
+		} else {
+			return -EFAULT;
+		}
+		a = hi;
+	}
+	return 0;
+}
+
+struct oimgpu_copy_chan {
+	int device = 0;
+	int sm_count = 0;
+	cudaStream_t stream = nullptr;
+	struct Op { cudaEvent_t ev; void *tag; };
+	std::deque<Op> inflight;
+	std::vector<cudaEvent_t> spare;
+	unsigned long long launches = 0;
+};
+
+extern "C" int oimgpu_copy_chan_open(int device, oimgpu_copy_chan **out)
+{
+	std::lock_guard<std::mutex> lk(g.mu);
+	if (!g.inited || g.control_only) return -ENODEV;
+	if (!out) return -EINVAL;
+	int d = device < 0 ? g.devices[0].ordinal : device;
+	const int slot = find_device_slot(d);
+	if (slot < 0) return -EINVAL;
+	auto c = std::make_unique<oimgpu_copy_chan>();
+	c->device = d;
+	c->sm_count = g.devices[slot].sm_count;
+	CU_OK(cudaSetDevice(d));
+	CU_OK(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
+	*out = c.release();
+	return 0;
+}
+
+extern "C" int oimgpu_copy_chan_close(oimgpu_copy_chan *c)
+{
+	if (!c) return -EINVAL;
+	cudaSetDevice(c->device);
+	cudaStreamSynchronize(c->stream);
+	for (auto &op : c->inflight) cudaEventDestroy(op.ev);
+	for (auto ev : c->spare) cudaEventDestroy(ev);
+	cudaStreamDestroy(c->stream);
+	delete c;
+	return 0;
+}
+
+static int chan_record(oimgpu_copy_chan *c, void *tag)
+{
+	cudaEvent_t ev;
+	if (!c->spare.empty()) { ev = c->spare.back(); c->spare.pop_back(); }
+	else CU_OK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+	CU_OK(cudaEventRecord(ev, c->stream));
+	c->inflight.push_back({ev, tag});
+	c->launches++;
+	return 0;
+}
+
+extern "C" int oimgpu_copy_chan_copy(oimgpu_copy_chan *c, void *dst, const void *src, uint64_t nbytes, void *tag)
+{
+	if (!c || !dst || !src) return -EINVAL;
+	int rc = oimgpu_mem_ensure(dst, nbytes);
+	if (rc == 0) rc = oimgpu_mem_ensure(src, nbytes);
+	if (rc) return rc;
+	CU_OK(cudaSetDevice(c->device));
+	if (nbytes) CU_OK(launch_copy(c->stream, c->sm_count, dst, src, nbytes));
+	return chan_record(c, tag);
+}
+
+extern "C" int oimgpu_copy_chan_fill(oimgpu_copy_chan *c, void *dst, uint8_t fill, uint64_t nbytes, void *tag)
+{
+	if (!c || !dst) return -EINVAL;
+	int rc = oimgpu_mem_ensure(dst, nbytes);
+	if (rc) return rc;
+	CU_OK(cudaSetDevice(c->device));
+	if (nbytes) CU_OK(launch_fill(c->stream, c->sm_count, dst, fill, nbytes));
+	return chan_record(c, tag);
+}
+
+extern "C" int oimgpu_copy_chan_poll(oimgpu_copy_chan *c, void **tags, int max)
+{
+	if (!c || (!tags && max > 0)) return -EINVAL;
+	int n = 0;
+	while (n < max && !c->inflight.empty()) {
+		cudaError_t e = cudaEventQuery(c->inflight.front().ev);
+		if (e == cudaErrorNotReady) { (void)cudaGetLastError(); break; }
+		if (e != cudaSuccess) { (void)cudaGetLastError(); return -EIO; }
+		tags[n++] = c->inflight.front().tag;
+		c->spare.push_back(c->inflight.front().ev);
+		c->inflight.pop_front();
+	}
+	return n;
+}
+
+extern "C" unsigned long long oimgpu_copy_chan_launches(const oimgpu_copy_chan *c) { return c ? c->launches : 0; }
