@@ -885,11 +885,11 @@ extern "C" int oimgpu_bdev_iostat(const char *name, oimgpu_iostat *out)
 	memcpy(sum, b->retired, sizeof(sum));
 	for (oimgpu_lun *L : g.handles) {
 		if (L->bdev == b->name && read_ctx_stats(L->device, L->d_ctx, v)) {
-			for (int k = 0; k < 8; k++) sum[k] += v[k];
+			for (int k = 0; k < 12; k++) sum[k] += v[k];
 		}
 		for (int t = 0; t < OIMGPU_CTRLR_MAX_DEVS; t++) {
 			if (L->peer_bdev[t] == b->name && read_ctx_stats(L->device, L->d_peer[t], v)) {
-				for (int k = 0; k < 8; k++) sum[k] += v[k];
+				for (int k = 0; k < 12; k++) sum[k] += v[k];
 			}
 		}
 	}

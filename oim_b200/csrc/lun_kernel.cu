@@ -503,13 +503,15 @@ __device__ __forceinline__ void parse_request(const LunCtx &L, const QueueDesc &
 		if ((cdb[1] & 0x1f) == 0x10) scsi_control(T, q, r, cnt, len, s, 2);
 		else set_check(s, SK_ILLEGAL_REQUEST, ASC_INVALID_OPCODE);
 		break;
-	case 0x35: case 0x91: {	/* SYNCHRONIZE CACHE: bounds check only; FLUSH is a no-op on a RAM disk */
+	case 0x35: case 0x91: {	/* SYNCHRONIZE CACHE: bounds check; the FLUSH is a no-op on a RAM disk, but a bdev_io all the same */
 		uint64_t lba; uint32_t n;
 		if (cdb[0] == 0x35) { lba = be32(&cdb[2]); n = be16(&cdb[7]); }
 		else { lba = be64(&cdb[2]); n = be32(&cdb[10]); }
 		if (n == 0) n = (uint32_t)(T.num_blocks - lba);
 		if (n != 0 && (lba >= T.num_blocks || n > T.num_blocks || lba > T.num_blocks - n)) {
 			set_check(s, SK_NO_SENSE, ASC_NONE);
+		} else if (n != 0) {
+			s.op = OP_FLUSH;	/* spdk_bdev_flush_blocks (scsi_bdev.c:1437) */
 		}
 		break;
 	}
@@ -1567,14 +1569,15 @@ __device__ __forceinline__ void tally_fill_latency(CtaShared &sh, const Stage &s
 		const uint32_t t = st.lat_tgt[i] & (OIMGPU_CTRLR_MAX_DEVS - 1);
 		unsigned long long *acc = sh.lat_ns[t];
 		acc[0] += dt * st.lat_n[i][0]; acc[1] += dt * st.lat_n[i][1]; acc[2] += dt * st.lat_n[i][2];
-		/* spdk_histogram_data_tally (histogram_data.h:120-160) of the fill's latency, once per request */
+		/* spdk_histogram_data_tally (histogram_data.h:120-160) of the fill's latency, once per bdev_io.  A latency
+		 * below the timer's resolution (dt == 0: __clzll gives 64) lands in bucket 0, so that no bdev_io goes untallied */
 		const LunCtx *T = (t == lun->target) ? lun : lun->peer[t];
 		unsigned long long *hist = T ? *reinterpret_cast<unsigned long long *const volatile *>(&T->hist) : nullptr;
-		if (hist && dt) {
+		if (hist) {
 			const uint32_t clz = (uint32_t)__clzll((long long)dt);
 			const uint32_t range = clz <= 57u ? 57u - clz : 0u;
 			const uint32_t index = (uint32_t)(dt >> (range ? range - 1 : 0)) & 127u;
-			atomicAdd(&hist[(range << 7) + index], (unsigned long long)(st.lat_n[i][0] + st.lat_n[i][1] + st.lat_n[i][2]));
+			atomicAdd(&hist[(range << 7) + index], (unsigned long long)(st.lat_n[i][0] + st.lat_n[i][1] + st.lat_n[i][2] + st.lat_n[i][3]));
 		}
 	}
 }
@@ -2067,21 +2070,27 @@ __device__ __forceinline__ void lun_queue_body(LunCtx *lun, KickHeader *hdr, con
 							st.vq_head[lane - r0] = (uint16_t)my_head;
 						}
 					}
-					/* latency accounting: the fill's good requests per target and kind (usually one target) */
+					/* latency accounting: the fill's bdev_ios per target and kind (usually one target).  A good READ, WRITE
+					 * or SYNCHRONIZE CACHE is one; an UNMAP is one per applied descriptor, whatever its final status */
 					{
-						uint32_t left = __ballot_sync(0xffffffffu, mine && good && s.op != OP_NONE);
+						const bool bios = mine && (s.op == OP_UNMAP ? s.resp_valid && s.response == OIMGPU_S_OK && s.nseg != 0
+											   : good && s.op != OP_NONE);
+						uint32_t left = __ballot_sync(0xffffffffu, bios);
 						uint32_t nt = 0;
 						while (left && nt < OIMGPU_CTRLR_MAX_DEVS) {
 							const uint32_t t = __shfl_sync(0xffffffffu, (uint32_t)s.tgt, __ffs(left) - 1);
-							const bool me = mine && good && s.op != OP_NONE && s.tgt == t;
+							const bool me = bios && s.tgt == t;
+							const uint32_t all = __ballot_sync(0xffffffffu, me);
 							const uint32_t rd = __ballot_sync(0xffffffffu, me && s.op == OP_READ);
 							const uint32_t wr = __ballot_sync(0xffffffffu, me && s.op == OP_WRITE);
-							const uint32_t um = __ballot_sync(0xffffffffu, me && s.op == OP_UNMAP);
+							const uint32_t fl = __ballot_sync(0xffffffffu, me && s.op == OP_FLUSH);
+							const uint32_t um = __reduce_add_sync(0xffffffffu, me && s.op == OP_UNMAP ? s.nseg : 0u);
 							if (lane == 0) {
 								st.lat_tgt[nt] = (uint8_t)t;
-								st.lat_n[nt][0] = (uint16_t)__popc(rd); st.lat_n[nt][1] = (uint16_t)__popc(wr); st.lat_n[nt][2] = (uint16_t)__popc(um);
+								st.lat_n[nt][0] = (uint16_t)__popc(rd); st.lat_n[nt][1] = (uint16_t)__popc(wr);
+								st.lat_n[nt][2] = (uint16_t)um; st.lat_n[nt][3] = (uint16_t)__popc(fl);
 							}
-							left &= ~(rd | wr | um);
+							left &= ~all;
 							nt++;
 						}
 						if (lane == 0) st.lat_ntgt = (uint8_t)nt;

@@ -59,7 +59,7 @@ constexpr int kMaxRegions = 8;			/* VHOST_MEMORY_MAX_NREGIONS */
 constexpr int kHistBuckets = 58 * 128;		/* SPDK_HISTOGRAM_NUM_BUCKETS at bucket_shift 7 (S/include/spdk/histogram_data.h:48-55) */
 constexpr int kIovRow = OIMGPU_IOVS_MAX + 1;	/* scratch SG row per parser lane in virtqueue mode */
 
-enum : uint8_t { OP_NONE = 0, OP_READ = 1, OP_WRITE = 2, OP_UNMAP = 3 };
+enum : uint8_t { OP_NONE = 0, OP_READ = 1, OP_WRITE = 2, OP_UNMAP = 3, OP_FLUSH = 4 };	/* OP_FLUSH: SYNCHRONIZE CACHE, no data */
 
 enum : uint8_t { SC_GOOD = 0x00, SC_CHECK = 0x02 };
 enum : uint8_t { SK_NO_SENSE = 0x0, SK_ILLEGAL_REQUEST = 0x5, SK_ABORTED_COMMAND = 0xb };
@@ -240,12 +240,13 @@ struct __align__(16) Stage {
 	uint32_t share_final;		/* launch + virtqueue: position at which the ring cursors are written back (count) */
 	uint32_t persistent;
 	uint32_t unit_ctr;		/* shared kernels: movers draw units from here (mover 0 also publishes, so it takes fewer) */
-	/* latency accounting (spdk_bdev_io_complete adds now - submit_tsc per I/O type, bdev.c:3316-3371): when the
-	 * pass was taken and how many of the fill's requests count as reads / writes / unmaps; mover warp 0 adds
-	 * (now - t0) x count when the fill's data has moved - the parser only stamps */
+	/* latency accounting (_spdk_bdev_io_complete, bdev.c:3233-3258, per completed bdev_io: the histogram tallies
+	 * every one, the latency sums only reads, writes and unmaps): when the pass was taken and how many bdev_ios of
+	 * each kind the fill's requests made; mover warp 0 adds (now - t0) x count when the fill's data has moved - the
+	 * parser only stamps */
 	uint64_t t0;
-	uint8_t  lat_ntgt, lat_tgt[OIMGPU_CTRLR_MAX_DEVS];	/* the SCSI targets the fill's good requests went to ... */
-	uint16_t lat_n[OIMGPU_CTRLR_MAX_DEVS][3];		/* ... and how many reads / writes / unmaps each */
+	uint8_t  lat_ntgt, lat_tgt[OIMGPU_CTRLR_MAX_DEVS];	/* the SCSI targets the fill's bdev_ios went to ... */
+	uint16_t lat_n[OIMGPU_CTRLR_MAX_DEVS][4];		/* ... and how many reads / writes / unmap descriptors / flushes each */
 };
 
 /* Store ranges of one pass, for hazard detection against the passes after it (parser-private).

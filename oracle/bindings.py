@@ -135,6 +135,21 @@ class _Oracle:
         gid.argtypes = [C.c_void_p, C.c_int]
         return gid(self.h, target)
 
+    IOSTAT_FIELDS = ("num_read_ops", "bytes_read", "num_write_ops", "bytes_written", "num_unmap_ops",
+                     "bytes_unmapped", "bdev_ios")
+
+    def iostat(self, target: int | None = None) -> dict:
+        """the target bdev's get_bdevs_iostat counters (oimgpu_iostat names) and, as bdev_ios, the total of its
+        latency histogram: one tally per completed bdev_io of any type and status"""
+        fn = getattr(self.lib, self.prefix + "_iostat")
+        fn.restype = C.c_int
+        fn.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_uint64)]
+        out = (C.c_uint64 * 7)()
+        rc = fn(self.h, self.target if target is None else target, out)
+        if rc != 0:
+            raise RuntimeError(f"{self.prefix}_iostat rc={rc}")
+        return dict(zip(self.IOSTAT_FIELDS, (int(v) for v in out)))
+
     def busy_ns(self, reset: bool = True) -> int:
         """ns spent inside the checker's own request processing (0 = not instrumented: time the call)"""
         return int(self._busy(self.h, int(reset)))
@@ -171,5 +186,11 @@ class PortOracle(_Oracle):
     prefix, path = "oimorc", PORT_SO
 
 
-def ref_available() -> bool:
-    return os.path.exists(REF_SO)
+def ref_available(*, iostat: bool = False) -> bool:
+    """oracle/_ref/liboim_ref.so is there.  iostat=True: and it exports the bdev counters (oimref_iostat).  Where the
+    reference sources are absent the library cannot be rebuilt, and one built before that export still serves every
+    other comparison; the counter comparisons then fall back to the restatement, which is pinned to the reference's
+    counters wherever the reference is present."""
+    if not os.path.exists(REF_SO):
+        return False
+    return not iostat or hasattr(C.CDLL(REF_SO), "oimref_iostat")

@@ -50,6 +50,9 @@ struct orc_bdev {
 	 * protocol identifier (vhost-scsi: SAS, vhost_scsi.c:1004-1013) */
 	char name[64], product_name[32], dev_name[16], port_name[16];
 	int  dev_id, port_index, protocol_id;
+	/* spdk_bdev_get_device_stat + the latency histogram's total (oimorc_iostat): num_read_ops, bytes_read,
+	 * num_write_ops, bytes_written, num_unmap_ops, bytes_unmapped, bdev_ios */
+	uint64_t stat[7];
 };
 
 /* per-session target state (struct spdk_scsi_dev_vhost_state, vhost_scsi.c:66-71) */
@@ -138,6 +141,18 @@ static bool bdev_valid_blocks(const struct orc_bdev *b, uint64_t off_blk, uint64
 	return true;
 }
 
+/* What _spdk_bdev_io_complete books for one completed bdev_io (S/lib/bdev/bdev.c:3236-3258): the histogram
+ * tallies every bdev_io whatever its type and status, the counters only successful reads, writes and unmaps.
+ * A request refused before a bdev_io exists (spdk_bdev_readv & co. returning -EINVAL) books nothing. */
+enum { IO_READ, IO_WRITE, IO_UNMAP, IO_FLUSH };
+static void bdev_io_complete(struct orc_bdev *b, int type, uint64_t nb, bool success)
+{
+	b->stat[6]++;
+	if (!success || type == IO_FLUSH) return;
+	b->stat[2 * type]++;
+	b->stat[2 * type + 1] += nb * b->blocklen;
+}
+
 /* bdev_malloc_check_iov_len (S/lib/bdev/malloc/bdev_malloc.c:137-150): fails only when the
  * iovecs are SHORTER than nbytes */
 static int malloc_check_iov_len(const struct orc_task *t, size_t nbytes)
@@ -161,12 +176,16 @@ static int bdev_readv(struct orc_bdev *b, struct orc_task *t, uint64_t offset, u
 
 	if (bdev_bytes_to_blocks(b, offset, &ob, nbytes, &nb) != 0) return -EINVAL;
 	if (!bdev_valid_blocks(b, ob, nb)) return -EINVAL;
-	if (malloc_check_iov_len(t, nb * b->blocklen)) return 1;
+	if (malloc_check_iov_len(t, nb * b->blocklen)) {
+		bdev_io_complete(b, IO_READ, nb, false);
+		return 1;
+	}
 	src = b->buf + ob * b->blocklen;
 	for (i = 0; i < t->iovcnt; i++) {
 		if (t->iovs[i].len) memcpy(t->iovs[i].base, src, t->iovs[i].len);
 		src += t->iovs[i].len;
 	}
+	bdev_io_complete(b, IO_READ, nb, true);
 	return 0;
 }
 
@@ -179,12 +198,16 @@ static int bdev_writev(struct orc_bdev *b, struct orc_task *t, uint64_t offset, 
 
 	if (bdev_bytes_to_blocks(b, offset, &ob, nbytes, &nb) != 0) return -EINVAL;
 	if (!bdev_valid_blocks(b, ob, nb)) return -EINVAL;
-	if (malloc_check_iov_len(t, nb * b->blocklen)) return 1;
+	if (malloc_check_iov_len(t, nb * b->blocklen)) {
+		bdev_io_complete(b, IO_WRITE, nb, false);
+		return 1;
+	}
 	dst = b->buf + ob * b->blocklen;
 	for (i = 0; i < t->iovcnt; i++) {
 		if (t->iovs[i].len) memcpy(dst, t->iovs[i].base, t->iovs[i].len);
 		dst += t->iovs[i].len;
 	}
+	bdev_io_complete(b, IO_WRITE, nb, true);
 	return 0;
 }
 
@@ -195,6 +218,7 @@ static int bdev_unmap_blocks(struct orc_bdev *b, uint64_t ob, uint64_t nb)
 	if (!bdev_valid_blocks(b, ob, nb)) return -EINVAL;
 	if (nb == 0) return -EINVAL;
 	memset(b->buf + ob * b->blocklen, 0, nb * b->blocklen);
+	bdev_io_complete(b, IO_UNMAP, nb, true);
 	return 0;
 }
 
@@ -267,7 +291,8 @@ static int scsi_readwrite(struct orc_bdev *b, struct orc_task *t, uint64_t lba, 
 	return is_read ? scsi_read(b, t, lba) : scsi_write(b, t, lba, xfer_len);
 }
 
-/* spdk_bdev_scsi_sync (scsi_bdev.c:1414-1454); Malloc FLUSH is a no-op success (bdev_malloc.c:235-241) */
+/* spdk_bdev_scsi_sync (scsi_bdev.c:1414-1454); Malloc FLUSH is a no-op success (bdev_malloc.c:235-241), but its
+ * bdev_io is tallied like any other */
 static int scsi_sync(struct orc_bdev *b, struct orc_task *t, uint64_t lba, uint32_t num_blocks)
 {
 	if (num_blocks == 0) return TASK_COMPLETE;
@@ -275,6 +300,7 @@ static int scsi_sync(struct orc_bdev *b, struct orc_task *t, uint64_t lba, uint3
 		task_set_status(t, SC_CHECK_CONDITION, SK_NO_SENSE, ASC_NONE, ASCQ_NONE);
 		return TASK_COMPLETE;
 	}
+	bdev_io_complete(b, IO_FLUSH, num_blocks, true);
 	t->data_transferred = 0;
 	return TASK_PENDING;
 }
@@ -1005,6 +1031,15 @@ int oimorc_scsi_dev_id(void *h, int target_num)
 }
 
 uint8_t *oimorc_store(void *h) { return ((struct oimorc *)h)->bdev.buf; }
+
+/* the target's bdev counters, in oimref_iostat's order; -ENODEV: no device in that slot */
+int oimorc_iostat(void *h, int target_num, uint64_t out[7])
+{
+	struct oimorc *o = h;
+	if (target_num < 0 || target_num >= OIMGPU_CTRLR_MAX_DEVS || !o->tgt[target_num].bdev) return -ENODEV;
+	memcpy(out, o->tgt[target_num].bdev->stat, sizeof(o->tgt[target_num].bdev->stat));
+	return 0;
+}
 uint64_t oimorc_num_blocks(void *h) { return ((struct oimorc *)h)->bdev.blockcnt; }
 
 void oimorc_set_removed(void *h, int target_num, int removed)

@@ -181,6 +181,20 @@ static int g_name_seq;
 
 static void init_done(void *arg, int rc) { *(int *)arg = rc ? -1 : 1; }
 
+/* the unit-test environment's tick counter (test_env.c:412-435).  It only moves when we move it: the driver
+ * advances it before it polls for completions, so every bdev_io takes at least one tick, as the histogram's
+ * tally requires (histogram_data.h:120-135 asserts a non-zero datapoint) */
+extern uint64_t ut_spdk_get_ticks;
+
+/* latency histogram on, as enable_bdev_histogram does it (bdev_rpc.c): every bdev_io of the bdev is tallied */
+static int ref_histogram_on(struct spdk_bdev *b)
+{
+	int done = 0;
+	spdk_bdev_histogram_enable(b, init_done, &done, true);
+	while (!done) spdk_thread_poll(g_thread, 0, 0);
+	return done < 0 ? -1 : 0;
+}
+
 static int ref_global_init(void)
 {
 	if (!g_lib_inited) {
@@ -247,6 +261,7 @@ static void *ref_create(const char *bdev_name, uint64_t num_blocks, uint32_t blo
 	else snprintf(r->bdev_name, sizeof(r->bdev_name), "RefMalloc%d", __sync_fetch_and_add(&g_name_seq, 1));
 	r->bdev = create_malloc_disk(r->bdev_name, NULL, num_blocks, block_size);
 	if (!r->bdev) { free(r); return NULL; }
+	if (ref_histogram_on(r->bdev) != 0) return NULL;
 
 	posix_memalign((void **)&r->svdev, 64, sizeof(*r->svdev));
 	memset(r->svdev, 0, sizeof(*r->svdev));
@@ -322,6 +337,7 @@ int oimref_add_target(void *h, const char *bdev_name, uint64_t num_blocks, uint3
 	}
 	b = create_malloc_disk(bdev_name, NULL, num_blocks, block_size);
 	if (!b) return -12;
+	if (ref_histogram_on(b) != 0) return -12;
 	names[0] = spdk_bdev_get_name(b);
 	snprintf(tname, sizeof(tname), "Target %d", target_num);
 	sdev = spdk_scsi_dev_construct(tname, names, lun_ids, 1, SPDK_SPC_PROTOCOL_IDENTIFIER_SAS, ref_hotremove_cb, r);
@@ -352,6 +368,54 @@ uint8_t *oimref_store(void *h)
 	/* struct malloc_disk { struct spdk_bdev disk; void *malloc_buf; ... } (bdev_malloc.c:50-54):
 	 * the bdev's ctxt is the malloc_disk, whose first member is the bdev itself. */
 	return *(uint8_t **)((char *)r->bdev->ctxt + sizeof(struct spdk_bdev));
+}
+
+static struct spdk_bdev *ref_target_bdev(struct oimref *r, int target_num)
+{
+	if (target_num < 0 || target_num >= SPDK_VHOST_SCSI_CTRLR_MAX_DEVS) return NULL;
+	if (r->extra[target_num]) return r->extra[target_num];
+	return r->svdev->scsi_dev_state[target_num].dev ? r->bdev : NULL;
+}
+
+static void stat_done(struct spdk_bdev *b, struct spdk_bdev_io_stat *stat, void *arg, int rc) { *(int *)arg = rc ? -1 : 1; }
+static void hist_done(void *arg, int rc, struct spdk_histogram_data *h) { *(int *)arg = rc ? -1 : 1; }
+static void hist_sum(void *ctx, uint64_t start, uint64_t end, uint64_t count, uint64_t total, uint64_t so_far)
+{
+	*(uint64_t *)ctx += count;
+}
+
+/* The target bdev's counters as get_bdevs_iostat reads them (spdk_bdev_get_device_stat, bdev_rpc.c:186) and the
+ * total of its latency histogram (spdk_bdev_histogram_get, as get_bdev_histogram): out = num_read_ops, bytes_read,
+ * num_write_ops, bytes_written, num_unmap_ops, bytes_unmapped, bdev_ios.  -ENODEV: no device in that slot. */
+int oimref_iostat(void *h, int target_num, uint64_t out[7])
+{
+	struct oimref *r = h;
+	struct spdk_bdev *b = ref_target_bdev(r, target_num);
+	struct spdk_bdev_io_stat stat;
+	struct spdk_histogram_data *hist;
+	int done = 0;
+
+	if (!b) return -ENODEV;
+	spdk_set_thread(g_thread);
+	memset(&stat, 0, sizeof(stat));
+	spdk_bdev_get_device_stat(b, &stat, stat_done, &done);
+	while (!done) spdk_thread_poll(g_thread, 0, 0);
+	if (done < 0) return -EIO;
+	out[0] = stat.num_read_ops;
+	out[1] = stat.bytes_read;
+	out[2] = stat.num_write_ops;
+	out[3] = stat.bytes_written;
+	out[4] = stat.num_unmap_ops;
+	out[5] = stat.bytes_unmapped;
+	hist = spdk_histogram_data_alloc();
+	if (!hist) return -ENOMEM;
+	done = 0;
+	spdk_bdev_histogram_get(b, hist, hist_done, &done);
+	while (!done) spdk_thread_poll(g_thread, 0, 0);
+	out[6] = 0;
+	if (done > 0) spdk_histogram_data_iterate(hist, hist_sum, &out[6]);
+	spdk_histogram_data_free(hist);
+	return done < 0 ? -EIO : 0;
 }
 
 uint64_t oimref_num_blocks(void *h) { return spdk_bdev_get_num_blocks(((struct oimref *)h)->bdev); }
@@ -478,6 +542,7 @@ int oimref_submit(void *h, const struct oimgpu_req *reqs, uint32_t nreqs,
 
 		clock_gettime(CLOCK_MONOTONIC, &t0);
 		process_requestq(r->svsession, r->vq);
+		ut_spdk_get_ticks++;
 		/* The Malloc module copies inline, but bdev.c defers the completion callback of an I/O
 		 * that finished inside submit_request to the next thread poll (bdev.c:3213-3229), so
 		 * successful I/Os reach the used ring after the pass, behind any request that failed
@@ -597,6 +662,7 @@ int oimref_vq_process(void *h, uint64_t desc, uint64_t avail, uint64_t used, uin
 	clock_gettime(CLOCK_MONOTONIC, &t0);
 	while ((uint16_t)(us->idx - start_used) != want && spins++ < 100000) {
 		process_requestq(r->svsession, vq);
+		ut_spdk_get_ticks++;
 		spdk_thread_poll(g_thread, 0, 0);
 		spdk_vhost_vq_used_signal(vs, vq);
 	}
@@ -625,20 +691,21 @@ static void ref_segv(int sig)
 	_exit(139);
 }
 
-extern uint64_t ut_spdk_get_ticks;
-
 void oimref_enter(void)
 {
 	ref_global_init();
 	spdk_set_thread(g_thread);
 }
 
-/* run the SPDK thread's pollers and messages (what a reactor iteration does) */
+/* run the SPDK thread's pollers and messages (what a reactor iteration does); a tick passes before each */
 void oimref_thread_poll(int iterations)
 {
 	int i;
 	spdk_set_thread(g_thread);
-	for (i = 0; i < iterations; i++) spdk_thread_poll(g_thread, 0, 0);
+	for (i = 0; i < iterations; i++) {
+		ut_spdk_get_ticks++;
+		spdk_thread_poll(g_thread, 0, 0);
+	}
 }
 
 const char *oimref_bdev_name(void *h) { return ((struct oimref *)h)->bdev_name; }

@@ -113,7 +113,8 @@ def _run_device_arrays(lun, reqs: np.ndarray, iovs: np.ndarray) -> np.ndarray:
 
 def run_cuda(lib, trace: traces.Trace, num_blocks: int, *, block_size: int = 512, store_seed: int | None = 7,
              arena_seed: int = 0x5EED, target: int = 0, mem: str = "device", removed: bool = False,
-             queue_size: int = 1024, name: str | None = None, kernel: str | None = None):
+             queue_size: int = 1024, name: str | None = None, kernel: str | None = None, histogram: bool = False,
+             lun_removed: bool = False):
     """Same replay through liboimgpu.so on cuda:0.  mem="device": client buffers in HBM (a torch
     tensor); mem="host": client buffers in pinned, registered host memory.
 
@@ -121,7 +122,10 @@ def run_cuda(lib, trace: traces.Trace, num_blocks: int, *, block_size: int = 512
     the library reports that it did (iostat kernel_launches, Lun.shared_launches).  The ring is sized to hold
     the trace (queue_size is then ignored); a trace longer than a ring goes in as device arrays.  One launch
     also keeps the write-mix switch (a write-hot session stops sharing) from changing the variant mid-trace.
-    The mirror variants put two replicas on cuda:0, and check that they end up equal."""
+    The mirror variants put two replicas on cuda:0, and check that they end up equal.
+
+    histogram: enable the bdev's latency histogram first; stats["histogram_total"] is then its number of tallies.
+    lun_removed: the session sees its LUN being torn down (every request aborted)."""
     import torch
     if kernel is not None:
         assert kernel in KERNELS, kernel
@@ -146,10 +150,12 @@ def run_cuda(lib, trace: traces.Trace, num_blocks: int, *, block_size: int = 512
                 lib.bdev_write_raw(bname, 0, init, replica=rep)
         if mirror:
             assert lib.get_bdevs(bname)[0]["replicas"] == 2
+        if histogram:
+            lib.enable_bdev_histogram(bname, True)
         with environ(**(kernel_env(kernel) if kernel is not None else {})), \
                 lib.Lun(cname, target, num_queues=1, queue_size=ring or 32) as lun:
-            if removed:
-                lun.set_removed(True)
+            if removed or lun_removed:
+                lun.set_removed(removed, lun_removed)
             if mem == "device":
                 dev = torch.from_numpy(host_arena).to("cuda:0")
                 base = dev.data_ptr()
@@ -164,6 +170,8 @@ def run_cuda(lib, trace: traces.Trace, num_blocks: int, *, block_size: int = 512
             torch.cuda.synchronize()
             arena = dev.cpu().numpy() if mem == "device" else pinned.numpy().copy()
             stats = lun.iostat()
+            if histogram:
+                stats["histogram_total"] = int(lib.get_bdev_histogram(bname).sum())
             if kernel is not None:
                 assert stats["kernel_launches"] == 1, f"kernel={kernel}: {stats['kernel_launches']} launches, expected 1"
                 shared = lun.shared_launches
