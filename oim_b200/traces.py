@@ -462,6 +462,192 @@ def alignment_sweep(num_blocks: int = 65536, *, block_size: int = 512, target: i
     return Trace(reqs, iovs, cursor[0] + 4096, "alignment-sweep", {"hazard_pass": len(reqs) // abi.REQS_PER_PASS - 2})
 
 
+# ------------------------------------------------------------------------------------------------
+# Block-size edges: the transfer limit, fills of more than kFillUnits units, READ(6) length 0, SG shapes and
+# UNMAP extents measured in blocks of any size.  Deterministic.
+# ------------------------------------------------------------------------------------------------
+
+FILL_BYTES = 1 << 20     # lun_kernel.cu kFillUnits x 4 KiB: a request above this has a fill of its own
+
+
+def block_size_trace(num_blocks: int, block_size: int, *, seed: int = 1, target: int = 0) -> Trace:
+    """The requests whose shape depends on the block size, in passes of abi.REQS_PER_PASS:
+
+    - READ/WRITE 6/10/12/16 at 1 block and at max = MAX_XFER_BYTES // block_size blocks (READ(6)/WRITE(6): at most
+      255), at LBA 0 and at the last fit, one past the last fit (LBA out of range) and max + 1 blocks (refused);
+    - READ(6)/WRITE(6) with length byte 0 (256 blocks) at LBA 0, num_blocks - 256 and num_blocks - 255;
+    - passes that mix requests over 1 MiB (FILL_BYTES) with one-block ones, the big one first, in the middle and last,
+      with hazards between them in the same and the next pass;
+    - SG lists of one element, of block-sized elements up to the 129-element limit and 130 (invalid), cut at odd bytes
+      inside a block, runs of elements that continue each other across 4 KiB, every client address mod 16, and a
+      pass of more than 256 segments;
+    - UNMAP of one many-MiB descriptor, of 256 one-block descriptors, a list that fails part-way and the whole
+      device, each followed by READs of what it unmapped in the same and the next pass;
+    - SYNCHRONIZE CACHE with count 0 from LBA 0 and near the end.
+
+    Passes are padded with READ CAPACITY 10/16, whose payloads carry the block size.  Addresses are arena offsets."""
+    bs, nb = block_size, num_blocks
+    mx = abi.MAX_XFER_BYTES // bs
+    assert bs >= 16 and nb >= 64 and nb < (1 << 21), "the 6-byte CDBs address the whole device"
+    rng = np.random.default_rng(seed)
+    b = abi.Batch(target)
+    cursor = [0]
+    pay = []
+
+    def buf(n: int, skew: int | None = None) -> int:
+        o = (cursor[0] + 127) // 64 * 64 + (int(rng.integers(0, 16)) if skew is None else skew)
+        cursor[0] = o + n
+        return o
+
+    def one(n: int, skew: int | None = None) -> list:
+        return [(buf(n, skew), n)]
+
+    stub = min(bs, 4096)                     # SG of a request refused before any data moves
+
+    def pad():
+        """READ CAPACITY 10 / 16 up to the next pass boundary"""
+        while len(b) % abi.REQS_PER_PASS:
+            six = len(b) % 2 == 0
+            b.add(abi.cdb_read_capacity(six, 32), abi.DIR_FROM_DEV, one(32 if six else 8))
+
+    def unmap(descs):
+        pl = abi.unmap_param_list(descs)
+        off = buf(len(pl))
+        pay.append((off, pl))
+        b.add(abi.cdb_unmap(len(pl)), abi.DIR_TO_DEV, [(off, len(pl))])
+
+    rd = {6: abi.READ_6, 10: abi.READ_10, 12: abi.READ_12, 16: abi.READ_16}
+    wr = {6: abi.WRITE_6, 10: abi.WRITE_10, 12: abi.WRITE_12, 16: abi.WRITE_16}
+
+    # every CDB width at 1 block and at the transfer limit, at both ends of the device
+    for width in (6, 10, 12, 16):
+        for d in (abi.DIR_FROM_DEV, abi.DIR_TO_DEV):
+            op = (rd if d == abi.DIR_FROM_DEV else wr)[width]
+            top = min(mx, 255) if width == 6 else mx
+            for n in sorted({1, top}):
+                for lba in sorted({0, nb - n}):
+                    b.add(abi.cdb_rw(op, lba, n), d, one(n * bs))
+                b.add(abi.cdb_rw(op, nb - n + 1, n), d, one(stub))
+            if width != 6 or mx + 1 <= 255:
+                b.add(abi.cdb_rw(op, 0, mx + 1), d, one(stub))
+
+    # READ(6) / WRITE(6) length byte 0: 256 blocks, or one block's SG where 256 blocks are over the limit
+    sg256 = 256 * bs if 256 <= mx else bs
+    for op, d in ((abi.READ_6, abi.DIR_FROM_DEV), (abi.WRITE_6, abi.DIR_TO_DEV)):
+        for lba in sorted({x for x in (0, nb - 256, nb - 255) if x >= 0}):
+            b.add(abi.cdb_rw(op, lba, 0), d, one(sg256))
+    b.add(abi.cdb_sync(abi.SYNCHRONIZE_CACHE_10, 0, 0), abi.DIR_FROM_DEV, [])
+    b.add(abi.cdb_sync(abi.SYNCHRONIZE_CACHE_16, nb - 4, 0), abi.DIR_FROM_DEV, [])
+    pad()
+
+    # passes mixing requests over one fill with one-block ones
+    big = max(1, (3 << 20) // bs)            # about 3 MiB
+    big2 = FILL_BYTES // bs + 1              # just over one fill
+    x, y, z = nb // 8, 3 * nb // 8, 5 * nb // 8
+    far = nb - nb // 8
+
+    def small(k, lo):
+        for i in range(k):
+            b.read(lo + (7 * i) % (nb // 8 - 1), 1, one(bs), opcode=abi.READ_16)
+
+    b.write(x, big, one(big * bs), opcode=abi.WRITE_16)           # big first: small READs inside it follow
+    for lba in (x, x + big // 2, x + big - 1):
+        b.read(lba, 1, one(bs), opcode=abi.READ_16)
+    small(3, far)
+    pad()
+    for lba in (x + big - 1, x + 1 if big > 1 else x):            # next pass: the big WRITE's blocks again
+        b.read(lba, 1, one(bs), opcode=abi.READ_16)
+    for i, lba in enumerate((y, y + big // 2, y + big - 1)):      # small WRITEs, then a big READ over them
+        b.write(lba, 1, one(bs, 3 * i + 1), opcode=abi.WRITE_16)
+    small(2, far)
+    b.read(y, big, one(big * bs), opcode=abi.READ_16)             # big in the middle
+    small(2, far)
+    pad()
+    small(3, far)
+    b.write(z, big2, one(big2 * bs), opcode=abi.WRITE_16)         # two big ones: a big WRITE over a big WRITE,
+    small(2, far)
+    b.write(z + big2 // 2, big2, one(big2 * bs), opcode=abi.WRITE_16)   # the second one last
+    pad()
+    b.read(z, big2 + big2 // 2, one((big2 + big2 // 2) * bs), opcode=abi.READ_16)
+    b.read(z + big2 // 2, 1, one(bs), opcode=abi.READ_16)
+    pad()
+
+    # SG shapes: block-sized elements up to the 129-element limit, 130 (invalid), odd cuts, runs across 4 KiB
+    sgl = x + big + 8
+    k = min(abi.IOVS_MAX, mx)
+    b.read(sgl, k, [(buf(bs, i % 16), bs) for i in range(k)], opcode=abi.READ_16)
+    b.write(sgl + k, k, [(buf(bs, (5 * i) % 16), bs) for i in range(k)], opcode=abi.WRITE_16)
+    n130 = abi.IOVS_MAX + 1
+    if n130 <= mx:
+        b.read(sgl, n130, [(buf(bs), bs) for i in range(n130)], opcode=abi.READ_16)
+    else:
+        cut = [bs // n130] * (n130 - 1)
+        b.read(sgl, 1, [(buf(c), c) for c in cut + [bs - sum(cut)]], opcode=abi.READ_16)
+    for d in (abi.DIR_FROM_DEV, abi.DIR_TO_DEV):                 # separate elements cut at odd bytes inside a block
+        nblk = 2 if 2 <= mx else 1
+        edges = sorted({0, 1, 7, bs - 3, bs + 5 if nblk > 1 else bs - 1, nblk * bs})
+        els = [(buf(e1 - e0), e1 - e0) for e0, e1 in zip(edges[:-1], edges[1:])]
+        (b.read if d == abi.DIR_FROM_DEV else b.write)(sgl + 2 * k + 4 * (d == abi.DIR_TO_DEV), nblk, els,
+                                                          opcode=abi.READ_16 if d == abi.DIR_FROM_DEV else abi.WRITE_16)
+    nrun = -(-20000 // bs)                                      # one buffer cut across 4 KiB: elements that continue
+    if nrun <= mx:
+        tot = nrun * bs
+        for d, skew in ((abi.DIR_TO_DEV, 9), (abi.DIR_FROM_DEV, 6)):
+            base = buf(tot, skew)
+            edges = sorted({e for e in (0, 4000, 4100, 8191, 8193, 12289, 16380) if e < tot} | {tot})
+            els = [(base + e0, e1 - e0) for e0, e1 in zip(edges[:-1], edges[1:])]
+            (b.read if d == abi.DIR_FROM_DEV else b.write)(sgl + 2 * k + 12, nrun, els, opcode=abi.READ_16 if d == abi.DIR_FROM_DEV else abi.WRITE_16)
+    pad()
+    many = max(1, -(-abi.IOVS_MAX * 64 // bs))                  # three requests of 129 separate elements: > 256 segments
+    tot = many * bs
+    cut = [tot // abi.IOVS_MAX] * (abi.IOVS_MAX - 1)
+    cut.append(tot - sum(cut))
+    seg0 = sgl + 2 * k + 40
+    for i in range(3):
+        els = [(buf(c), c) for c in cut]
+        if i == 1:
+            b.write(seg0 + i * many, many, els, opcode=abi.WRITE_16)
+        else:
+            b.read(seg0 + i * many, many, els, opcode=abi.READ_16)
+    b.read(seg0 + many, many, one(tot), opcode=abi.READ_16)      # what the WRITE of 129 elements left
+    pad()
+
+    # UNMAP: a many-MiB descriptor, 256 one-block descriptors, a list that fails part-way; then reads of them
+    u = nb // 2
+    ucnt = min(nb // 8, max(2, (8 << 20) // bs))
+    v = (u + ucnt + 4) % nb
+    w = (v + 520) % (nb - 8)
+    unmap([(u, ucnt)])
+    b.read(u, 1, one(bs), opcode=abi.READ_16)
+    b.read(u + ucnt - 1, 1, one(bs), opcode=abi.READ_16)
+    unmap([((v + 2 * i) % nb, 1) for i in range(256)])
+    b.read(v, min(4, mx), one(min(4, mx) * bs), opcode=abi.READ_16)
+    unmap([(w, 2), (nb - 1, 4), (w + 4, 2)])
+    b.read(w, 1, one(bs), opcode=abi.READ_16)
+    pad()
+    two = min(2, mx)
+    b.read(u + 1 - two, two, one(two * bs), opcode=abi.READ_16)   # across the start and the end of the extent
+    b.read(u + ucnt - 1, two, one(two * bs), opcode=abi.READ_16)
+    b.read((v + 2) % nb, 1, one(bs), opcode=abi.READ_16)
+    b.read(w, min(6, mx), one(min(6, mx) * bs), opcode=abi.READ_16)
+    pad()
+
+    # the whole device, then reads of it and writes after it
+    unmap([(0, nb)])
+    b.read(0, 1, one(bs), opcode=abi.READ_16)
+    b.read(nb - 1, 1, one(bs), opcode=abi.READ_16)
+    pad()
+    b.read(nb // 2, min(2, mx), one(min(2, mx) * bs), opcode=abi.READ_16)
+    b.write(1, min(3, mx), one(min(3, mx) * bs), opcode=abi.WRITE_16)
+    b.write(nb - mx, mx, one(mx * bs), opcode=abi.WRITE_16)
+    b.read(0, min(4, mx), one(min(4, mx) * bs), opcode=abi.READ_16)
+    pad()
+    reqs, iovs = b.arrays()
+    t = Trace(reqs, iovs, cursor[0] + 4096, f"block-size-{bs}", {"n": len(reqs)})
+    t.meta["param_payloads"] = pay
+    return t
+
+
 def _param_iovs(alloc, payload: np.ndarray, rng) -> list[tuple[int, int]]:
     """SG list for a TO_DEV parameter list (UNMAP): one element, or cut in two at a ragged spot."""
     n = len(payload)

@@ -66,18 +66,19 @@ def test_multi_target_restatement_matches_reference(oracles, seed, kind):
 
 
 class Controller:
-    """three Malloc bdevs on one controller, as MapVolume x3 leaves them"""
+    """three Malloc bdevs on one controller, as MapVolume x3 leaves them.  sizes: {target: (blocks, block size)}"""
 
-    def __init__(self, gpu, only=None):
+    def __init__(self, gpu, only=None, sizes=None):
         self.gpu = gpu
+        self.sizes = sizes or {t: (TARGETS[t], 512) for t in TARGETS}
         tag = next(_seq)
         self.ctrlr = f"mtc{tag}"
         self.names = {t: f"mtb{tag}_{t}" for t in TARGETS}
         gpu.construct_vhost_scsi_controller(self.ctrlr)
         self.attached = set()
-        for t in TARGETS:
-            gpu.construct_malloc_bdev(TARGETS[t], 512, name=self.names[t], device=0)
-            gpu.bdev_write_raw(self.names[t], 0, traces.pattern_bytes(7 + (t if t != 1 else 0), 0, TARGETS[t] * 512))
+        for t, (nb, bs) in self.sizes.items():
+            gpu.construct_malloc_bdev(nb, bs, name=self.names[t], device=0)
+            gpu.bdev_write_raw(self.names[t], 0, traces.pattern_bytes(7 + (t if t != 1 else 0), 0, nb * bs))
             if only is None or t in only:
                 self.attach(t)
 
@@ -93,7 +94,7 @@ class Controller:
         return {x["scsi_dev_num"]: x["id"] for x in self.gpu.get_vhost_controllers(self.ctrlr)[0]["backend_specific"]["scsi"]}
 
     def stores(self):
-        return {t: self.gpu.bdev_read_raw(self.names[t], 0, TARGETS[t] * 512) for t in TARGETS}
+        return {t: self.gpu.bdev_read_raw(self.names[t], 0, nb * bs) for t, (nb, bs) in self.sizes.items()}
 
     def close(self):
         for t in list(self.attached):

@@ -1,5 +1,6 @@
 """The trace generators the parity tests and bench.py's SG legs rely on (host logic, CPU only)."""
 import numpy as np
+import pytest
 
 import util
 from oim_b200 import abi, traces, vring
@@ -93,6 +94,157 @@ def test_alignment_sweep_covers_every_skew_and_edge(oracles):
     assert lbas[p + abi.REQS_PER_PASS][:2] == w[:2], "pass p + 1: a read of what pass p wrote"
     cpls = util.run_oracle(oracles.PortOracle, t, nb)[0]
     assert (cpls["status"] == 0).all() and (cpls["resid"] == 0).all(), "every request of the sweep is a good one"
+
+
+BLOCK_SIZES = (520, 1000, 4097, 4160, 1024, 2048, 4096, 8192, 16384, 32768, 1 << 20, 4 << 20)
+RW = {abi.READ_6: 6, abi.WRITE_6: 6, abi.READ_10: 10, abi.WRITE_10: 10, abi.READ_12: 12, abi.WRITE_12: 12,
+      abi.READ_16: 16, abi.WRITE_16: 16}
+
+
+def decode(t, arena):
+    """one record per request: opcode, CDB width, LBA, blocks (READ(6) length 0 = 256), SG elements, pass, and the
+    UNMAP descriptors read back from the parameter list in the arena"""
+    out = []
+    for i, r in enumerate(t.reqs):
+        c = bytes(r["cdb"])
+        iov = t.iovs[int(r["iov_start"]):int(r["iov_start"]) + int(r["iovcnt"])]
+        rec = {"i": i, "op": c[0], "width": RW.get(c[0]), "pass": i // abi.REQS_PER_PASS, "iov": iov,
+               "len0": False, "descs": []}
+        if rec["width"] == 6:
+            rec["lba"], rec["n"], rec["len0"] = int.from_bytes(c[1:4], "big") & 0x1FFFFF, c[4] or 256, c[4] == 0
+        elif rec["width"] in (10, 12):
+            rec["lba"] = int.from_bytes(c[2:6], "big")
+            rec["n"] = int.from_bytes(c[7:9], "big") if rec["width"] == 10 else int.from_bytes(c[6:10], "big")
+        elif rec["width"] == 16 or c[0] == abi.SYNCHRONIZE_CACHE_16:
+            rec["lba"], rec["n"] = int.from_bytes(c[2:10], "big"), int.from_bytes(c[10:14], "big")
+        elif c[0] == abi.SYNCHRONIZE_CACHE_10:
+            rec["lba"], rec["n"] = int.from_bytes(c[2:6], "big"), int.from_bytes(c[7:9], "big")
+        elif c[0] == abi.UNMAP:
+            pl = np.concatenate([arena[int(a):int(a) + int(n)] for a, n in zip(iov["addr"], iov["len"])])
+            rec["descs"] = [(int.from_bytes(bytes(pl[8 + 16 * k:16 + 16 * k]), "big"),
+                             int.from_bytes(bytes(pl[16 + 16 * k:20 + 16 * k]), "big"))
+                            for k in range(int.from_bytes(bytes(pl[2:4]), "big") // 16)]
+        out.append(rec)
+    return out
+
+
+def segments(rec) -> int:
+    """the mover's segments of one request: non-empty elements that do not continue their predecessor, or one per
+    UNMAP descriptor"""
+    if rec["descs"]:
+        return sum(1 for _, n in rec["descs"] if n)
+    iov = rec["iov"][rec["iov"]["len"] > 0]
+    return len(iov) - int(continues(iov).sum()) if len(iov) else 0
+
+
+@pytest.mark.parametrize("bs", BLOCK_SIZES)
+def test_block_size_trace_covers_every_edge(oracles, bs):
+    """traces.block_size_trace: each case is there, and the reference (or the restatement pinned to it) gives it the
+    status it is in the trace for"""
+    nb = (256 << 20) // bs
+    mx = abi.MAX_XFER_BYTES // bs
+    t = traces.block_size_trace(nb, bs)
+    assert len(t.reqs) > abi.REQS_PER_PASS and len(t.reqs) % abi.REQS_PER_PASS == 0
+    cls = oracles.RefOracle if oracles.ref_available() else oracles.PortOracle
+    cpls, arena, _ = util.run_oracle(cls, t, nb, block_size=bs)
+    arena0 = np.zeros(t.arena_bytes, dtype=np.uint8)
+    traces.fill_arena(arena0, t)
+    recs = decode(t, arena0)
+    good = (cpls["resp_valid"] == 1) & (cpls["response"] == abi.S_OK) & (cpls["status"] == abi.STATUS_GOOD)
+
+    def sense(i):
+        return int(cpls["sense"][i][2]) & 0xF, int(cpls["sense"][i][12])
+
+    def moved(rec):
+        return good[rec["i"]] and cpls["resid"][rec["i"]] == 0 and int(rec["iov"]["len"].sum()) == rec["n"] * bs
+
+    rw = [r for r in recs if r["width"]]
+    reads = {abi.READ_6, abi.READ_10, abi.READ_12, abi.READ_16}
+    for width in (6, 10, 12, 16):
+        for is_read in (True, False):
+            mine = [r for r in rw if r["width"] == width and (r["op"] in reads) == is_read and not r["len0"]]
+            top = min(mx, 255) if width == 6 else mx
+            for n in (1, top):
+                for lba in (0, nb - n):
+                    assert any(r["n"] == n and r["lba"] == lba and moved(r) for r in mine), (width, is_read, n, lba)
+                oor = [r for r in mine if r["n"] == n and r["lba"] == nb - n + 1]
+                assert oor and all(sense(r["i"]) == (abi.SK_ILLEGAL_REQUEST, abi.ASC_LBA_OUT_OF_RANGE) for r in oor)
+            if width != 6 or mx + 1 <= 255:
+                over = [r for r in mine if r["n"] == mx + 1]
+                assert over and all(sense(r["i"]) == (abi.SK_ILLEGAL_REQUEST, abi.ASC_INVALID_FIELD_IN_CDB) for r in over)
+    # READ(6) / WRITE(6) with length byte 0: 256 blocks where they fit, refused where they are over the limit
+    for op in (abi.READ_6, abi.WRITE_6):
+        l0 = {r["lba"]: r for r in rw if r["len0"] and r["op"] == op}
+        if nb >= 256:
+            want = None if 256 <= mx else (abi.SK_ILLEGAL_REQUEST, abi.ASC_INVALID_FIELD_IN_CDB)
+            for lba in (0, nb - 256):
+                assert moved(l0[lba]) if want is None else sense(l0[lba]["i"]) == want, (op, lba)
+            assert sense(l0[nb - 255]["i"]) == (abi.SK_ILLEGAL_REQUEST, abi.ASC_LBA_OUT_OF_RANGE)
+        else:
+            assert sense(l0[0]["i"]) == (abi.SK_ILLEGAL_REQUEST, abi.ASC_LBA_OUT_OF_RANGE)
+    # passes that mix requests over one fill with one-block ones: the big one first, in the middle and last
+    data = [r for r in rw if moved(r)]
+    bigs = {r["i"] for r in data if r["n"] * bs > traces.FILL_BYTES}
+    where = set()
+    for p in {r["pass"] for r in data if r["i"] in bigs}:
+        inp = [r for r in data if r["pass"] == p]
+        for k, r in enumerate(inp):                   # (at 4 MiB one block is over a fill: big and small at once)
+            if r["i"] in bigs and sum(1 for o in inp if o["n"] == 1 and o["i"] != r["i"]) >= 2:
+                where.add("first" if k == 0 else "last" if k == len(inp) - 1 else "middle")
+    assert where == {"first", "middle", "last"}, where
+
+    def over(a, c):
+        return a["lba"] < c["lba"] + c["n"] and c["lba"] < a["lba"] + a["n"]
+
+    def after(first, then, same):
+        return [(a, c) for a in data for c in data if a["i"] < c["i"] and over(a, c) and first(a) and then(c)
+                and (a["pass"] == c["pass"]) == same and c["pass"] - a["pass"] <= 1]
+    is_w = lambda r: r["op"] not in reads     # noqa: E731
+    big = lambda r: r["i"] in bigs            # noqa: E731
+    small = lambda r: r["n"] == 1             # noqa: E731
+    for same in (True, False):
+        assert after(lambda a: big(a) and is_w(a), lambda c: small(c) and not is_w(c), same), "big WRITE, small READ"
+    assert after(lambda a: small(a) and is_w(a), lambda c: big(c) and not is_w(c), True), "small WRITE, big READ"
+    assert after(lambda a: big(a) and is_w(a), lambda c: big(c) and is_w(c), True), "big WRITE over a big WRITE"
+    # SG shapes
+    k = min(abi.IOVS_MAX, mx)
+    assert any(len(r["iov"]) == 1 for r in data)
+    assert any(len(r["iov"]) == k and (r["iov"]["len"] == bs).all() for r in data), "block-sized elements to the limit"
+    too_many = [r for r in rw if len(r["iov"]) == abi.IOVS_MAX + 1]
+    assert too_many and not any(good[r["i"]] for r in too_many)
+
+    def offsets(r):
+        return np.concatenate([[0], np.cumsum(r["iov"]["len"].astype(np.int64))[:-1]])
+    assert any(((offsets(r) % bs) % 2 == 1).any() for r in data), "an element starting at an odd byte of a block"
+    assert any(((offsets(r)[1:][continues(r["iov"])] % 4096) != 0).any() and segments(r) < len(r["iov"])
+               and (offsets(r) + r["iov"]["len"] > 4096).any() for r in data if len(r["iov"]) > 2), \
+        "a run of elements that continue each other across a 4 KiB unit"
+    assert {int(a) % 16 for r in data for a in r["iov"]["addr"]} == set(range(16))
+    per_pass = {}
+    for r in recs:
+        if good[r["i"]]:
+            per_pass[r["pass"]] = per_pass.get(r["pass"], 0) + segments(r)
+    assert max(per_pass.values()) > 256, "a pass of more than kSegCap segments"
+    # UNMAP and the READs behind it
+    unmaps = [r for r in recs if r["op"] == abi.UNMAP]
+    ok_unmaps = [r for r in unmaps if good[r["i"]]]
+    assert any(len(r["descs"]) == 1 and r["descs"][0][1] * bs > traces.FILL_BYTES for r in ok_unmaps)
+    assert any(r["descs"] == [(0, nb)] for r in ok_unmaps)
+    assert any(len(r["descs"]) == 256 and all(n == 1 for _, n in r["descs"]) for r in ok_unmaps)
+    part = [r for r in unmaps if not good[r["i"]] and r["descs"][0][0] + r["descs"][0][1] <= nb
+            and any(a + n > nb for a, n in r["descs"][1:])]
+    assert part and all(cpls["status"][r["i"]] == abi.STATUS_CHECK_CONDITION for r in part), "UNMAP failing part-way"
+    for same in (True, False):
+        hit = [(u, r) for u in unmaps for r in data if r["op"] in reads and r["i"] > u["i"]
+               and (r["pass"] == u["pass"]) == same and r["pass"] - u["pass"] <= 1
+               and any(over(r, {"lba": a, "n": n}) for a, n in u["descs"])]
+        assert len({u["i"] for u, _ in hit}) == len(unmaps), f"a READ of every UNMAP's blocks (same pass: {same})"
+    # SYNCHRONIZE CACHE with count 0 from LBA 0 and near the end; READ CAPACITY
+    syncs = [r for r in recs if r["op"] in (abi.SYNCHRONIZE_CACHE_10, abi.SYNCHRONIZE_CACHE_16) and good[r["i"]]]
+    assert {r["lba"] for r in syncs if r["n"] == 0} >= {0, nb - 4}
+    rc = {int(t.reqs["cdb"][r["i"]][0]) for r in recs if good[r["i"]]}
+    assert {abi.READ_CAPACITY_10, abi.SERVICE_ACTION_IN_16} <= rc
+    assert (arena != arena0).any()
 
 
 def test_guest_images_with_runs_of_contiguous_descriptors():

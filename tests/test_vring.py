@@ -16,17 +16,21 @@ VQ_KERNELS = {
 }
 
 
-def make_requests(seed: int, n: int = 96, nb: int = 32768, contiguous: bool = False):
-    t = traces.fuzz_trace(n, nb, seed=seed, max_io_blocks=[8, 64, 300][seed % 3], arena_bytes=16 << 20, contiguous=contiguous)
+def make_requests(seed: int, n: int = 96, nb: int = 32768, contiguous: bool = False, block_size: int = 512):
+    """a fuzz trace as guest requests; at other block sizes the largest transfer keeps its size in bytes, so that a
+    kick's data still fits the guest image"""
+    mx = max(1, [8, 64, 300][seed % 3] * 512 // block_size)
+    t = traces.fuzz_trace(n, nb, block_size=block_size, seed=seed, max_io_blocks=mx, arena_bytes=16 << 20,
+                          contiguous=contiguous)
     a0 = np.zeros(t.arena_bytes, dtype=np.uint8)
     traces.fill_arena(a0, t)
     return vring.requests_from_trace(t, a0)
 
 
-def run_kicks_oracle(cls, rq, nb, ring_size, seed, mutate=True, contiguous=False):
+def run_kicks_oracle(cls, rq, nb, ring_size, seed, mutate=True, contiguous=False, block_size=512):
     """replay `rq` in as many kicks as the ring needs; -> [(masked image, sorted used entries, cursors)], store"""
     out = []
-    with cls(nb) as o:
+    with cls(nb, block_size) as o:
         o.store[:] = traces.pattern_bytes(7, 0, o.store.size)
         pos = kick = 0
         while pos < len(rq):
