@@ -1146,11 +1146,7 @@ __device__ __forceinline__ void reap_stage(Stage &st, int lane, QShare **pub_q =
 	if (st.vq_in_hbm) __threadfence();
 	else __threadfence_system();
 	__syncwarp();
-	if (lane == 0 && n) {
-		const uint32_t idx = st.used_base + n;
-		*reinterpret_cast<volatile uint16_t *>(st.vq_used + 2) = (uint16_t)idx;
-		if (!st.share) st.vq_state->last_used = idx & 0xffff;
-	}
+	if (lane == 0 && n) *reinterpret_cast<volatile uint16_t *>(st.vq_used + 2) = (uint16_t)(st.used_base + n);
 	if (st.share && lane == 0) {
 		if (!st.persistent && st.share_pos + n == st.share_final) {
 			/* last fill of this launch on the queue: everything before it is published - write the cursors back */
@@ -1871,7 +1867,9 @@ __device__ __forceinline__ void lun_queue_body(LunCtx *lun, KickHeader *hdr, con
 			int4 vq_raw = make_int4(0, 0, 0, 0);	/* desc[head] of the coming pass, still in flight */
 			const bool vq_tbl_aligned = ((uintptr_t)q.vq_desc & 15) == 0;
 			if (!shared && q.count && q.mode == QMODE_VRING && (uint32_t)lane < min((uint32_t)kPass, q.count)) {
-				vq_head_cur = reinterpret_cast<const uint16_t *>(q.vq_avail + 4)[(q.head + lane) & (q.vq_size - 1)];
+				/* volatile, as every avail entry read: a resident CTA has this line in its L1 from the batch before,
+				 * when the guest had not written these entries yet */
+				vq_head_cur = reinterpret_cast<const volatile uint16_t *>(q.vq_avail + 4)[(q.head + lane) & (q.vq_size - 1)];
 				if (vq_tbl_aligned && vq_head_cur < q.vq_size) vq_raw = ld_cg16(q.vq_desc + (size_t)vq_head_cur * 16);
 			}
 			uint32_t done = 0;	/* position of the current pass on the queue */
@@ -2130,7 +2128,13 @@ __device__ __forceinline__ void lun_queue_body(LunCtx *lun, KickHeader *hdr, con
 				}
 				vq_head_cur = vq_head_nxt;
 			}
-			if (!shared && q.mode == QMODE_VRING && lane == 0) q.vq_state->last_avail = (vq_last_avail + q.count) & 0xffff;
+			if (!shared && q.mode == QMODE_VRING && lane == 0) {
+				/* the parser owns both cursors: every consumed avail entry has its used element at vq_last_used + its
+				 * position, published or not.  A resident CTA that comes straight back to this ring while the movers
+				 * still hold the batch must place the next one behind it, not where publication has got to */
+				q.vq_state->last_avail = (vq_last_avail + q.count) & 0xffff;
+				q.vq_state->last_used = (vq_last_used + q.count) & 0xffff;
+			}
 			if (!shared && persistent && q.mode == QMODE_SLOTS && lane == 0) q.vq_state->last_avail = q.head + q.count;
 		}
 		/* tell the movers to stop, then publish the completions still in flight */

@@ -23,6 +23,7 @@ F_NEXT, F_WRITE, F_INDIRECT = 1, 2, 4
 desc_dtype = np.dtype([("addr", "<u8"), ("len", "<u4"), ("flags", "<u2"), ("next", "<u2")])
 used_elem_dtype = np.dtype([("id", "<u4"), ("len", "<u4")])
 MB2 = 2 << 20
+USED_SENTINEL = 0xA5C3_5A3C      # both words of every used element nobody has written yet
 
 # guest-physical layout: two 4 MiB regions that are adjacent in GPA but swapped in the arena (so a
 # buffer crossing 0x600000 is NOT contiguous in VA and must be split, vhost.c:481-500), then one big
@@ -66,6 +67,18 @@ class GuestImage:
         ring = a[self.used_off + 4:self.used_off + 4 + 8 * self.ring_size].view(used_elem_dtype)
         return idx, ring
 
+    def used_in_order(self, arena: np.ndarray | None, start_used: int, n: int) -> np.ndarray:
+        """the n used elements from ring position start_used on, in ring order (they wrap at the ring's end)"""
+        ring = self.used_entries(arena)[1]
+        return ring[(start_used + np.arange(n)) & (self.ring_size - 1)]
+
+    def used_untouched(self, arena: np.ndarray, start_used: int, n: int) -> bool:
+        """every used element outside the n from start_used on still holds USED_SENTINEL"""
+        ring = self.used_entries(arena)[1].view("<u4").reshape(-1, 2)
+        keep = np.ones(self.ring_size, dtype=bool)
+        keep[(start_used + np.arange(n)) & (self.ring_size - 1)] = False
+        return bool((ring[keep] == USED_SENTINEL).all())
+
     def masked(self, arena: np.ndarray) -> np.ndarray:
         """copy of an arena with the used ring's element area zeroed (its order is timing-dependent
         in the reference); the used idx stays"""
@@ -87,11 +100,17 @@ class _Alloc:
 
 
 def build_image(requests: list[dict], *, ring_size: int = 256, data_bytes: int = 24 << 20, seed: int = 0,
-                mutate: bool = True, pattern_seed: int = 0x5EED, contiguous: bool = False) -> GuestImage:
+                mutate: bool = True, pattern_seed: int = 0x5EED, contiguous: bool = False, start_avail: int = 0,
+                start_used: int = 0, all_indirect: bool = False) -> GuestImage:
     """requests: [{'cdb','dir','lun','tag','sg': [len,...], 'payload': optional bytes for TO_DEV}]
     One kick's worth: at most ring_size requests.
     contiguous: a request's data elements are cuts of one guest buffer (each continues its predecessor, with an
-    occasional gap) instead of separate buffers."""
+    occasional gap) instead of separate buffers.
+    start_avail / start_used: the ring cursors the device resumes from.  The requests sit at avail positions
+    (start_avail + i) mod ring_size, avail->idx = start_avail + n and used->idx = start_used (both mod 2^16).  The
+    avail entries outside that window hold random descriptor indices below ring_size, so a device that reads the
+    wrong entry serves a wrong but plausible chain; every used element holds USED_SENTINEL until it is written.
+    all_indirect: every chain is one INDIRECT ring slot, so the ring holds ring_size requests."""
     rng = np.random.default_rng(seed)
     r2_size = (4 << 20) + data_bytes
     arena = np.zeros(2 * R01_SIZE + r2_size, dtype=np.uint8)
@@ -123,7 +142,7 @@ def build_image(requests: list[dict], *, ring_size: int = 256, data_bytes: int =
 
     placed = 0
     for rq in requests[:ring_size]:
-        if len(free) < 4:
+        if len(free) < (1 if all_indirect else 4):
             break                                      # ring full: the rest goes into the next kick
         placed += 1
         sg_lens = list(rq["sg"])
@@ -206,7 +225,7 @@ def build_image(requests: list[dict], *, ring_size: int = 256, data_bytes: int =
             j = (2 if from_dev else 1) + int(rng.integers(0, len(data_descs)))
             chain[j] = (R2_GPA + r2_size - 100, max(chain[j][1], 4096), chain[j][2])   # runs off the end of a region
 
-        use_indirect = len(chain) > len(free) - 3 or (mutate and rng.integers(0, 3) == 0) or len(chain) > 40
+        use_indirect = all_indirect or len(chain) > len(free) - 3 or (mutate and rng.integers(0, 3) == 0) or len(chain) > 40
         if use_indirect:
             tbl_off = meta.take(16 * len(chain), 16)
             tbl = arena[tbl_off:tbl_off + 16 * len(chain)].view(desc_dtype)
@@ -233,13 +252,22 @@ def build_image(requests: list[dict], *, ring_size: int = 256, data_bytes: int =
             head = idxs[0]
         if kind == 13:
             head = ring_size + int(rng.integers(0, 100))              # avail entry beyond the ring
-        avail_ring[n_avail] = head
+        avail_ring[(start_avail + n_avail) & (ring_size - 1)] = head
         n_avail += 1
         img.heads.append(head)
         notes.append(kind)
-    arena[avail_off + 2:avail_off + 4] = np.frombuffer(np.uint16(n_avail).tobytes(), dtype=np.uint8)
+    # what lies outside the published window comes from a generator of its own: at cursor 0 an image keeps the
+    # draws it always had
+    rest = np.random.default_rng([seed, 0xA7A1])
+    outside = np.ones(ring_size, dtype=bool)
+    outside[(start_avail + np.arange(n_avail)) & (ring_size - 1)] = False
+    avail_ring[outside] = rest.integers(0, ring_size, int(outside.sum()))
+    img.used_entries()[1].view("<u4")[:] = USED_SENTINEL
+    arena[avail_off + 2:avail_off + 4] = np.frombuffer(np.uint16((start_avail + n_avail) & 0xFFFF).tobytes(), dtype=np.uint8)
+    arena[used_off + 2:used_off + 4] = np.frombuffer(np.uint16(start_used & 0xFFFF).tobytes(), dtype=np.uint8)
     img.meta["kinds"] = notes
     img.meta["placed"] = placed
+    img.meta["start"] = (start_avail & 0xFFFF, start_used & 0xFFFF)
     return img
 
 

@@ -252,9 +252,9 @@ def test_cuda_vring_block_sizes(gpu, oracles, kernel, bs):
                 assert lun.shared_launches - shared == (kernel == "shared"), f"kick {kick} did not take the {kernel} kernel"
                 la, lu = lun.vq_detach(0)
                 after = dev.cpu().numpy()
-                idx, uring = img.used_entries(after)
+                used = img.used_in_order(after, 0, img.used_entries(after)[0])
                 assert (la, lu) == w[kick][2][1:], f"kick {kick}: cursors"
-                assert sorted((int(i), int(n)) for i, n in uring[:idx]) == w[kick][1], f"kick {kick}: used elements"
+                assert sorted((int(i), int(n)) for i, n in used) == w[kick][1], f"kick {kick}: used elements"
                 got = img.masked(after)
                 assert (got == w[kick][0]).all(), f"kick {kick}: guest memory differs at {np.nonzero(got != w[kick][0])[0][:8]}"
                 pos += img.meta["placed"]

@@ -7,9 +7,14 @@ import pytest
 
 import util
 from oim_b200 import abi, traces, vring
+from test_vring import VQ_KERNELS
 
 pytestmark = pytest.mark.gpu
 WATCHDOG_MS = 4000
+# the resident kernel a single guest ring of 256 runs on: the shared-queue kernel (default); with
+# OIMGPU_NO_SHARED_QUEUES=1 oim_lun_vring_kernel, where mover warp 0 publishes; with OIMGPU_NO_VRING_KERNEL=1 as well,
+# oim_lun_queue_kernel, where the parser publishes
+POLLER_VARIANTS = VQ_KERNELS
 
 
 def _setup(gpu, name, nb):
@@ -258,6 +263,167 @@ def test_slot_ring_passes_that_straddle_the_ring_end(gpu, oracles, resident):
                     lun.stop_poller()
         util.assert_cpls_equal(np.concatenate(got), want, t.reqs)
         assert (arena.numpy() == oa).all()
+        assert (gpu.bdev_read_raw(name, 0, nb * 512) == want_store).all()
+    finally:
+        _teardown(gpu, name)
+
+
+def _wait_used(used_idx, target, what, timeout_s=20.0):
+    deadline = time.time() + timeout_s
+    while int(used_idx[0]) != target and time.time() < deadline:
+        time.sleep(0.0005)
+    assert int(used_idx[0]) == target, f"{what}: used->idx is {int(used_idx[0])} after {timeout_s:.0f} s, expected {target}"
+
+
+@pytest.mark.timeout(180)
+@pytest.mark.parametrize("variant", list(POLLER_VARIANTS))
+def test_poller_guest_ring_across_the_index_wrap(gpu, oracles, variant):
+    """test_poller_guest_reuses_ring_and_buffers from cursor 65536 - 100: rounds of 40 requests carry avail->idx and
+    used->idx across the 16-bit wrap and the ring's end under the resident kernel.  After stop_poller the cursors
+    vq_detach returns are the oracle's, mod 2^16."""
+    import torch
+    nb, rounds, per, R = 32768, 5, 40, 256
+    start = 65536 - 100
+    imgs, refs, cur = [], [], []
+    with oracles.PortOracle(nb) as o:
+        o.store[:] = traces.pattern_bytes(7, 0, o.store.size)
+        la = lu = start
+        for r in range(rounds):
+            t = traces.fuzz_trace(per, nb, seed=950 + r, max_io_blocks=32, arena_bytes=8 << 20, include_malformed=False)
+            a0 = np.zeros(t.arena_bytes, dtype=np.uint8)
+            traces.fill_arena(a0, t)
+            rq = vring.requests_from_trace(t, a0)
+            kw = dict(ring_size=R, seed=3, mutate=False, pattern_seed=0x5EED + r, start_avail=la, start_used=lu)
+            img, ref = vring.build_image(rq, **kw), vring.build_image(rq, **kw)
+            assert img.meta["placed"] == per
+            cur.append((la, lu))
+            n, la, lu = o.vq_process(ref, la, lu)
+            assert n == per
+            imgs.append(img)
+            refs.append(ref)
+        want_store = o.store.copy()
+        want_cursors = (la, lu)
+    assert want_cursors == ((start + rounds * per) & 0xFFFF,) * 2
+    name = f"pvw{variant}"
+    _setup(gpu, name, nb)
+    try:
+        img0 = imgs[0]
+        guest = torch.from_numpy(img0.arena.copy()).pin_memory()
+        g = guest.numpy()
+        avail_idx = g[img0.avail_off + 2:img0.avail_off + 4].view("<u2")
+        used_idx = g[img0.used_off + 2:img0.used_off + 4].view("<u2")
+        avail_idx[0] = start                                   # nothing published yet
+        base = guest.data_ptr()
+        lo, hi = img0.avail_off, img0.used_off + 4 + 8 * R
+        with util.environ(**POLLER_VARIANTS[variant]), gpu.Lun(f"{name}.ctl", 0, num_queues=1, queue_size=32) as lun:
+            lun.set_mem_table(img0.region_table(base))
+            lun.vq_attach(0, base + img0.desc_off, base + img0.avail_off, base + img0.used_off, R, start, start)
+            shared = lun.shared_launches
+            lun.start_poller(idle_timeout_ms=WATCHDOG_MS)
+            try:
+                assert lun.shared_launches - shared == (variant == "shared"), f"the poller is not the {variant} kernel"
+                for r in range(rounds):
+                    img, (la, lu) = imgs[r], cur[r]
+                    if r:
+                        # the guest rewrites its memory in place, then the avail entries of this round's window
+                        g[:lo] = img.arena[:lo]
+                        g[hi:] = img.arena[hi:]
+                        ring = g[img.avail_off + 4:img.avail_off + 4 + 2 * R].view("<u2")
+                        src = img.arena[img.avail_off + 4:img.avail_off + 4 + 2 * R].view("<u2")
+                        pos = (la + np.arange(per)) & (R - 1)
+                        ring[pos] = src[pos]
+                    assert int(used_idx[0]) == lu
+                    avail_idx[0] = (la + per) & 0xFFFF
+                    _wait_used(used_idx, (lu + per) & 0xFFFF, f"round {r} (from {la},{lu})")
+                    used = img.used_in_order(g, lu, per)
+                    assert [int(i) for i in used["id"]] == img.heads, f"round {r}: used elements out of ring order"
+                    assert sorted((int(i), int(l)) for i, l in used) == \
+                        sorted((int(i), int(l)) for i, l in refs[r].used_in_order(None, lu, per)), f"round {r}: used elements"
+                    want = refs[r].arena
+                    assert (g[:lo] == want[:lo]).all(), f"round {r}: guest memory differs at {np.nonzero(g[:lo] != want[:lo])[0][:8]}"
+                    assert (g[hi:] == want[hi:]).all(), f"round {r}: guest memory differs at {hi + np.nonzero(g[hi:] != want[hi:])[0][:8]}"
+            finally:
+                lun.stop_poller()
+            assert lun.vq_detach(0) == want_cursors
+        assert (gpu.bdev_read_raw(name, 0, nb * 512) == want_store).all()
+    finally:
+        _teardown(gpu, name)
+
+
+def _spin_us(us: float) -> None:
+    t = time.perf_counter() + us * 1e-6
+    while time.perf_counter() < t:
+        pass
+
+
+@pytest.mark.timeout(180)
+@pytest.mark.parametrize("variant", list(POLLER_VARIANTS))
+def test_poller_guest_publishes_while_a_batch_moves(gpu, oracles, variant):
+    """A Linux guest bumps avail->idx for every request it adds, so the resident kernel finds new requests on a ring
+    while the batch before them is still moving.  First 32 READs of 1 MiB into guest memory (pinned host memory:
+    around a millisecond of PCIe traffic, estimated), then the rest of a fuzz trace one request at a time - avail
+    entry, then avail->idx + 1, tens of microseconds apart - including writes to the blocks the READs read.  From
+    cursor 65536 - 50, so the batches also cross the 16-bit wrap.  Everything equals the oracle's single pass over the
+    same image: used->idx, the used elements in ring order, guest memory, store, and the cursors after stop."""
+    import torch
+    nb, R, big = 32768, 256, 2048
+    start = 65536 - 50
+    rng = np.random.default_rng(61)
+    reads = []
+    for k in range(32):
+        cdb = np.zeros(32, dtype=np.uint8)
+        c = abi.cdb_rw(abi.READ_10, int(rng.integers(0, nb - big)), big)
+        cdb[:len(c)] = c
+        reads.append({"cdb": cdb, "dir": abi.DIR_FROM_DEV, "lun": abi.virtio_lun(0), "tag": 0x7000 + k,
+                      "sg": [big * 512], "payload": None})
+    t = traces.fuzz_trace(96, nb, seed=62, max_io_blocks=64, arena_bytes=8 << 20, include_malformed=False)
+    a0 = np.zeros(t.arena_bytes, dtype=np.uint8)
+    traces.fill_arena(a0, t)
+    rq = reads + vring.requests_from_trace(t, a0)
+    n = len(rq)
+    kw = dict(ring_size=R, seed=4, mutate=False, all_indirect=True, data_bytes=48 << 20, start_avail=start, start_used=start)
+    img, ref = vring.build_image(rq, **kw), vring.build_image(rq, **kw)
+    assert img.meta["placed"] == n
+    end = (start + n) & 0xFFFF
+    with oracles.PortOracle(nb) as o:
+        o.store[:] = traces.pattern_bytes(7, 0, o.store.size)
+        assert o.vq_process(ref, start, start) == (n, end, end)
+        want_store = o.store.copy()
+    name = f"pvs{variant}"
+    _setup(gpu, name, nb)
+    try:
+        guest = torch.from_numpy(img.arena.copy()).pin_memory()
+        g = guest.numpy()
+        avail_idx = g[img.avail_off + 2:img.avail_off + 4].view("<u2")
+        used_idx = g[img.used_off + 2:img.used_off + 4].view("<u2")
+        ring = g[img.avail_off + 4:img.avail_off + 4 + 2 * R].view("<u2")
+        pos = (start + np.arange(n)) & (R - 1)
+        ring[pos[32:]] = (ring[pos[32:]] + 1) % R             # not yet written by the guest: wrong heads
+        avail_idx[0] = start
+        base = guest.data_ptr()
+        with util.environ(**POLLER_VARIANTS[variant]), gpu.Lun(f"{name}.ctl", 0, num_queues=1, queue_size=32) as lun:
+            lun.set_mem_table(img.region_table(base))
+            lun.vq_attach(0, base + img.desc_off, base + img.avail_off, base + img.used_off, R, start, start)
+            shared = lun.shared_launches
+            lun.start_poller(idle_timeout_ms=WATCHDOG_MS)
+            try:
+                assert lun.shared_launches - shared == (variant == "shared"), f"the poller is not the {variant} kernel"
+                avail_idx[0] = (start + 32) & 0xFFFF               # the 32 large READs
+                for k in range(32, n):
+                    _spin_us(30)
+                    ring[pos[k]] = img.heads[k]                    # the avail entry, then the index that publishes it
+                    avail_idx[0] = (start + k + 1) & 0xFFFF
+                _wait_used(used_idx, end, f"{n} requests published one by one from {start}")
+            finally:
+                lun.stop_poller()
+            cursors = lun.vq_detach(0)
+        used = img.used_in_order(g, start, n)
+        assert [int(i) for i in used["id"]] == img.heads, "used elements out of ring order"
+        assert sorted((int(i), int(l)) for i, l in used) == sorted((int(i), int(l)) for i, l in ref.used_in_order(None, start, n))
+        assert img.used_untouched(g, start, n), "a used element outside the published window was written"
+        got, want = img.masked(g.copy()), ref.masked(ref.arena)
+        assert (got == want).all(), f"guest memory differs at {np.nonzero(got != want)[0][:8]}"
+        assert cursors == (end, end)
         assert (gpu.bdev_read_raw(name, 0, nb * 512) == want_store).all()
     finally:
         _teardown(gpu, name)

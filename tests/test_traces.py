@@ -263,3 +263,49 @@ def test_guest_images_with_runs_of_contiguous_descriptors():
         counts[contiguous] = adj
     # (request headers and response buffers are packed next to each other in both images: the difference is the data)
     assert counts[True] > counts[False] + 30, counts
+
+
+@pytest.mark.parametrize("ring", [64, 256, 1024])
+@pytest.mark.parametrize("case", ["zero", "ring-end", "wrap-mid", "wrap-pass", "split"])
+def test_guest_images_reach_the_cursor_cases(case, ring):
+    """vring.build_image(start_avail=, start_used=) over the kicks of test_vring's replay: every request sits at its
+    avail position, the indices say what the window holds, the rest of the avail ring holds plausible heads and the
+    used elements the sentinel - and the crossing each cursor case names happens between two requests of one kick,
+    at the request it names (on rings of 256 and up, whose first kick holds the first passes: at the pass position)"""
+    from test_vring import CURSOR_CASES, kick_images, make_requests
+    seed = 440 + list(CURSOR_CASES).index(case)
+    rq = make_requests(seed)
+    start = CURSOR_CASES[case](ring)
+    seen = {}                    # crossing -> (kick, request of the replay, request of the kick)
+    g0 = 0
+    for k, (img, (la, lu)) in enumerate(kick_images(rq, ring, seed, start=start)):
+        n = img.meta["placed"]
+        avail = img.arena[img.avail_off + 4:img.avail_off + 4 + 2 * ring].view("<u2")
+        pos = (la + np.arange(n)) & (ring - 1)
+        assert [int(h) for h in avail[pos]] == img.heads, f"kick {k}: requests not at their avail positions"
+        outside = np.ones(ring, dtype=bool)
+        outside[pos] = False
+        assert (avail[outside] < ring).all()
+        assert img.avail_idx == (la + n) & 0xFFFF and img.used_entries()[0] == lu
+        assert img.used_untouched(img.arena, lu, 0)
+        for i in range(1, n):
+            for which, c in (("avail", la), ("used", lu)):
+                if (c + i) % ring == 0:
+                    seen.setdefault(f"{which} ring end", (k, g0 + i, i))
+                if (c + i) % 65536 == 0:
+                    seen.setdefault(f"{which} wrap", (k, g0 + i, i))
+        g0 += n
+    assert g0 == len(rq)
+    named = {"zero": {}, "ring-end": {"avail ring end": 7, "used ring end": 7},
+             "wrap-mid": {"avail wrap": 45, "used wrap": 45}, "wrap-pass": {"avail wrap": 32, "used wrap": 32},
+             "split": {"avail wrap": 6, "used ring end": ring - 1000 % ring}}[case]
+    for what, g in named.items():
+        assert what in seen and seen[what][1] == g, f"{what}: {seen.get(what)}, expected at request {g}"
+    if case == "zero":
+        assert not any("wrap" in w for w in seen)
+    if case == "ring-end":
+        assert seen["avail ring end"][0] == 0
+    if ring >= 256 and case in ("wrap-mid", "wrap-pass"):
+        kick, _, i = seen["avail wrap"]
+        assert kick == 0 and i // abi.REQS_PER_PASS == 1
+        assert (i % abi.REQS_PER_PASS == 0) == (case == "wrap-pass")

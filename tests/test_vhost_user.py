@@ -103,7 +103,8 @@ def publish(ram, ring, heads):
     ram.mem[a_off + 2:a_off + 4] = np.frombuffer(struct.pack("<H", idx & 0xFFFF), np.uint8)
 
 
-def handshake(m: vu.Master, ram, img, queues):
+def handshake(m: vu.Master, ram, img, queues, bases=None):
+    """bases: the SET_VRING_BASE value of each queue (default 0)"""
     f = m.get_u64(vu.GET_FEATURES)
     pf = m.get_u64(vu.GET_PROTOCOL_FEATURES)
     m.set_u64(vu.SET_PROTOCOL_FEATURES, pf & ((1 << vu.PF_MQ) | (1 << vu.PF_REPLY_ACK)))
@@ -113,8 +114,8 @@ def handshake(m: vu.Master, ram, img, queues):
     m.set_u64(vu.SET_FEATURES, f & ~(1 << vu.F_LOG_ALL), need_reply=True)
     regs = [(g, s, vu.UVA_BASE + o, o, ram.fd) for g, s, o in img.regions]
     assert m.set_mem_table(regs, need_reply=True) == 0
-    for q in queues:                                    # in index order, as QEMU does
-        q.setup(m)
+    for k, q in enumerate(queues):                      # in index order, as QEMU does
+        q.setup(m, bases[k] if bases else 0)
         m.vring_state(vu.SET_VRING_ENABLE, q.index, 1)
     return f, pf
 
@@ -243,9 +244,75 @@ def mask(mem, img, rings):
     return c
 
 
-def used_set(mem, ring, n):
-    u = mem[ring[2] + 4:ring[2] + 4 + 8 * n].view(vring.used_elem_dtype)
-    return sorted((int(i), int(l)) for i, l in u)
+def used_set(mem, ring, n, start=0, size=16):
+    """the n used elements of a small ring from position start on (they wrap at the ring's end), as a set"""
+    u = mem[ring[2] + 4:ring[2] + 4 + 8 * size].view(vring.used_elem_dtype)
+    return sorted((int(i), int(l)) for i, l in u[(start + np.arange(n)) % size])
+
+
+def resume_script(s: Slave, rq, *, base: int, used_idx: int, seed=5):
+    """A VM that hands its rings over with SET_VRING_BASE `base` while its RAM says used->idx = avail->idx = used_idx
+    on every ring (QEMU resuming a guest that has run for a while).  The control queue then serves its 8 requests and
+    the request queue (2) the image's requests in two notifies, the first 30 and the rest.  Near the 16-bit wrap the
+    control queue's requests cross it, and so does the second notify's batch.  -> (transcript, guest memory, image, rings, GET_VRING_BASE of every queue)"""
+    img = vring.build_image(rq, ring_size=256, seed=seed, mutate=False, start_avail=used_idx, start_used=used_idx)
+    n = img.meta["placed"] if rq else 0
+    ram = vu.GuestRam(img.arena.size)
+    ram.mem[:] = img.arena
+    cq, eq, q3 = small_ring(0), small_ring(1), small_ring(2)
+    idx = np.frombuffer(struct.pack("<H", used_idx & 0xFFFF), np.uint8)
+    for r in (cq, eq, q3):
+        ram.mem[r[0]:r[0] + 8192] = 0
+        ram.mem[r[1] + 2:r[1] + 4] = idx
+        ram.mem[r[2] + 2:r[2] + 4] = idx
+    ram.mem[img.avail_off + 2:img.avail_off + 4] = idx         # nothing of the image published yet
+    queues = [vu.Queue(0, 16, *cq[:3]), vu.Queue(1, 16, *eq[:3]), vu.Queue(2, img.ring_size, img.desc_off, img.avail_off, img.used_off),
+              vu.Queue(3, 16, *q3[:3])]
+    m = vu.Master(s.sock("scsi0"))
+    try:
+        handshake(m, ram, img, queues, bases=[base] * len(queues))
+        deadline, pending = time.time() + 10, list(queues)
+        while pending and time.time() < deadline:
+            pending = [q for q in pending if q.drain_calls() < 1]
+            time.sleep(0.02)
+        assert not pending, "every queue gets a spurious interrupt at start (vhost.c:1101-1115)"
+        time.sleep(0.2)
+        publish(ram, cq, control_requests(ram, img, cq))
+        queues[0].notify()
+        wait_used(ram, cq, (used_idx + 8) & 0xFFFF)
+        a_off = img.avail_off + 2
+        for upto in sorted({min(30, n), n} - {0}):
+            ram.mem[a_off:a_off + 2] = np.frombuffer(struct.pack("<H", (used_idx + upto) & 0xFFFF), np.uint8)
+            queues[2].notify()
+            queues[2].wait_used(ram, used_idx + upto)
+        mem = ram.mem.copy()
+        bases = [m.get_vring_base(q.index) for q in queues]
+        return m.log, mem, img, (cq, eq, q3), bases
+    finally:
+        m.close()
+        for q in queues:
+            q.close()
+        ram.close()
+
+
+def check_resume(ours, ref, rq, base, used_idx):
+    """resume_script against both slaves: the same transcript (GET_VRING_BASE replies included), the same guest
+    memory and used elements, every ring resumed at used->idx"""
+    lo, mo, img, rings, bo = resume_script(ours, rq, base=base, used_idx=used_idx)
+    lr, mr, _, _, br = resume_script(ref, rq, base=base, used_idx=used_idx)
+    assert deliberate(lo) == deliberate(lr), f"protocol transcripts differ:\nours {lo}\nref  {lr}"
+    n = img.meta["placed"] if rq else 0
+    assert bo == br == [(used_idx + 8) & 0xFFFF, used_idx, (used_idx + n) & 0xFFFF, used_idx], (bo, br)
+    a, b = mask(mo, img, rings), mask(mr, img, rings)
+    assert (a == b).all(), f"guest memory differs at {np.nonzero(a != b)[0][:16]}"
+    cq = rings[0]
+    assert used_set(mo, cq, 8, used_idx) == used_set(mr, cq, 8, used_idx)
+    assert sorted(h for h, _ in used_set(mo, cq, 8, used_idx)) == list(range(0, 16, 2))
+    if n:
+        uo, ur = img.used_in_order(mo, used_idx, n), img.used_in_order(mr, used_idx, n)
+        assert sorted((int(i), int(l)) for i, l in uo) == sorted((int(i), int(l)) for i, l in ur)
+        assert sorted(int(i) for i in uo["id"]) == sorted(img.heads)
+        assert img.used_untouched(mo, used_idx, n) and img.used_untouched(mr, used_idx, n)
 
 
 @pytest.fixture()
@@ -334,6 +401,15 @@ def test_vhost_user_reconnect_and_odd_masters(slaves):
     assert not os.path.exists(ours.sock("scsi0"))
 
 
+@pytest.mark.parametrize("base,used_idx", [(65530, 65530), (0, 65500)], ids=["base-65530", "base-0-used-65500"])
+def test_vhost_user_resumes_at_the_guests_used_index(slaves, base, used_idx):
+    """SET_VRING_BASE near the 16-bit wrap, and SET_VRING_BASE 0 on rings whose used->idx says 65500: both slaves
+    resume at used->idx (vhost_user.c:337-453), the control queue's requests cross the wrap, and the GET_VRING_BASE
+    replies are the same, byte for byte"""
+    ours, ref = slaves("ours", ["--control-only"]), slaves("ref")
+    check_resume(ours, ref, [], base, used_idx)
+
+
 def make_requests(seed, n=96):
     t = traces.fuzz_trace(n, NB, seed=seed, max_io_blocks=64, arena_bytes=16 << 20)
     a0 = np.zeros(t.arena_bytes, dtype=np.uint8)
@@ -375,6 +451,16 @@ def test_cuda_vhost_user_io_matches_reference(slaves, mode):
     assert raw["read_latency_ticks"] > 0 and raw["write_latency_ticks"] > 0, raw      # summed by the mover warps, 1 GHz ticks
     m0 = [x for x in a if x.get("name") == "M0"][0]
     assert m0["num_read_ops"] > 0 and m0["num_write_ops"] > 0 and [x for x in a if x.get("name") == "M1"][0]["num_read_ops"] == 1
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("mode", ["kick", "poller"])
+def test_cuda_vhost_user_io_from_a_high_base(slaves, mode):
+    """SET_VRING_BASE 65500 with the guest image built at that cursor: the request queue's I/O comes in two notifies
+    and crosses the 16-bit wrap; guest memory, transcript and GET_VRING_BASE equal the reference's transport"""
+    ours, ref = slaves("ours", ["--poller"] if mode == "poller" else []), slaves("ref")
+    rq = make_requests(12, n=80)
+    check_resume(ours, ref, rq, 65500, 65500)
 
 
 class Vm:
