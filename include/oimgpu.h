@@ -384,6 +384,50 @@ unsigned long long oimgpu_copy_chan_launches(const oimgpu_copy_chan *chan);	/* k
  * registered parts are skipped); -EFAULT if the range cannot be pinned */
 int oimgpu_mem_ensure(const void *addr, size_t len);
 
+/* ---- block-I/O channel (one level above the copy engine: struct spdk_bdev_fn_table) ---------------------
+ * Block I/O with caller iovecs on one HBM-resident oimgpu bdev, for an SPDK bdev module
+ * (integration/spdk/bdev_oimgpu.c) whose submit_request hands its bdev_ios over in batches.  No SCSI:
+ * no 4 MiB transfer cap, no 129-element SG cap.  One oim_bio_kernel launch serves a whole batch (more when
+ * the batch holds overlapping I/Os one of which writes: each launch then ends before the next one starts).
+ * Requests of one channel take effect in submission order wherever ranges overlap and one of them writes;
+ * different channels are mutually unordered.  iovecs point into device memory or ordinary host memory, which
+ * is pinned on first use (oimgpu_mem_ensure).  The buffers of an I/O belong to the channel until it completes.
+ * The bdev's own counters (oimgpu_bdev_iostat) do not count these I/Os: the bdev layer above does. */
+#define OIMGPU_BIO_READ			0
+#define OIMGPU_BIO_WRITE		1
+#define OIMGPU_BIO_WRITE_ZEROES		2	/* fills with 0x00 */
+#define OIMGPU_BIO_UNMAP		3	/* fills with 0x00, as bdev_malloc_unmap does (bdev_malloc.c:222-233) */
+
+struct oimgpu_bio {
+	uint64_t offset_blocks;
+	uint64_t num_blocks;
+	uint32_t op;		/* OIMGPU_BIO_* */
+	uint32_t iov_start;	/* READ / WRITE: first element in the iovec table passed with the batch */
+	uint32_t iovcnt;
+	uint32_t flags;		/* reserved, must be 0 */
+	uint64_t tag;
+};
+
+struct oimgpu_bio_cpl {
+	uint64_t tag;
+	int32_t  status;	/* 0 or -errno: -EINVAL for a bio outside the bdev, a bad op, iovecs out of the table or
+				 * READ / WRITE iovecs summing to fewer bytes than the bio; -EFAULT if an iovec could
+				 * not be made accessible to the GPU.  A failed bio moves nothing. */
+	uint32_t pad;
+};
+
+typedef struct oimgpu_bio_chan oimgpu_bio_chan;
+/* -ENODEV no GPU or no such bdev, -ENOTSUP mirrored bdev.  The bdev cannot be deleted (-EBUSY) while a channel is open. */
+int oimgpu_bio_chan_open(const char *bdev_name, oimgpu_bio_chan **out);
+/* Asynchronous: returns once the batch is enqueued.  Exactly num_blocks x block_size bytes move per bio, even where
+ * its iovecs hold more.  Returns 0, or -errno when nothing of the batch was taken (-EINVAL: NULL arguments). */
+int oimgpu_bio_chan_submit(oimgpu_bio_chan *chan, const struct oimgpu_bio *bios, uint32_t n,
+			   const struct oimgpu_iov *iovs, uint32_t niovs);
+/* completions in submission order; returns how many (<= max), 0 if none yet */
+int oimgpu_bio_chan_poll(oimgpu_bio_chan *chan, struct oimgpu_bio_cpl *out, int max);
+int oimgpu_bio_chan_close(oimgpu_bio_chan *chan);		/* waits for what is in flight */
+unsigned long long oimgpu_bio_chan_launches(const oimgpu_bio_chan *chan);	/* oim_bio_kernel launches so far */
+
 #ifdef __cplusplus
 }
 #endif

@@ -61,6 +61,13 @@ cpl_dtype = np.dtype([
 ])
 assert req_dtype.itemsize == 64 and iov_dtype.itemsize == 16 and cpl_dtype.itemsize == 48
 
+# block-I/O channel (oimgpu_bio_chan): one bio and its completion
+BIO_READ, BIO_WRITE, BIO_WRITE_ZEROES, BIO_UNMAP = 0, 1, 2, 3
+bio_dtype = np.dtype([("offset_blocks", "<u8"), ("num_blocks", "<u8"), ("op", "<u4"), ("iov_start", "<u4"),
+                      ("iovcnt", "<u4"), ("flags", "<u4"), ("tag", "<u8")])
+bio_cpl_dtype = np.dtype([("tag", "<u8"), ("status", "<i4"), ("pad", "<u4")])
+assert bio_dtype.itemsize == 40 and bio_cpl_dtype.itemsize == 16
+
 # completion fields the reference defines (everything but our bookkeeping extras)
 CPL_PARITY_FIELDS = ("tag", "sense_len", "resid", "status_qualifier", "status", "response",
                      "sense", "resp_valid", "used_len")

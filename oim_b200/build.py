@@ -12,7 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "liboimgpu.so")
-SOURCES = ["control.cu", "session.cu", "nbd.cu", "copy_chan.cu", "lun_kernel.cu"]
+SOURCES = ["control.cu", "session.cu", "nbd.cu", "copy_chan.cu", "bio_chan.cu", "lun_kernel.cu"]
 HEADERS = ["host_state.h", "lun_kernel.cuh", os.path.join(ROOT, "include", "oimgpu.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",

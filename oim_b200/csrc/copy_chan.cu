@@ -67,12 +67,60 @@ void oimgpu::unpin_all_host_ranges()
 	g_pinned.clear();
 }
 
-static bool pin_range(uintptr_t a, uintptr_t b)
+bool oimgpu::host_range_pinned(const void *addr, size_t len)
+{
+	const uintptr_t a = (uintptr_t)addr;
+	{
+		std::lock_guard<std::mutex> lk(g_pin_mu);
+		auto it = g_pinned.upper_bound(a);
+		if (it != g_pinned.begin() && std::prev(it)->first <= a && a + len <= std::prev(it)->second) return true;
+	}
+	std::lock_guard<std::mutex> lk(g.mu);
+	auto it = g.registered.upper_bound((void *)addr);
+	return it != g.registered.begin() && (uintptr_t)std::prev(it)->first + std::prev(it)->second >= a + len;
+}
+
+enum PinResult { PIN_NEW, PIN_FOREIGN, PIN_FAIL };
+
+static PinResult pin_range(uintptr_t a, uintptr_t b)
 {
 	cudaError_t e = cudaHostRegister((void *)a, b - a, cudaHostRegisterMapped | cudaHostRegisterPortable);
-	if (e == cudaSuccess) return true;
+	if (e == cudaSuccess) return PIN_NEW;
 	(void)cudaGetLastError();
-	return e == cudaErrorHostMemoryAlreadyRegistered;	/* by someone else (cudaHostAlloc, oimgpu_mem_register): fine */
+	/* registered by someone else (cudaHostAlloc, oimgpu_mem_register) - theirs to keep or let go */
+	return e == cudaErrorHostMemoryAlreadyRegistered ? PIN_FOREIGN : PIN_FAIL;
+}
+
+int oimgpu::pin_host_pages(const void *addr, size_t len)
+{
+	const uintptr_t page = 4096, big = 2u << 20;
+	uintptr_t a = (uintptr_t)addr & ~(page - 1), b = ((uintptr_t)addr + len + page - 1) & ~(page - 1);
+	std::lock_guard<std::mutex> lk(g_pin_mu);
+	/* walk the gaps between what is already pinned */
+	while (a < b) {
+		auto it = g_pinned.upper_bound(a);
+		if (it != g_pinned.begin()) {
+			auto pv = std::prev(it);
+			if (pv->second > a) { a = pv->second; continue; }	/* inside a pinned range: skip it */
+		}
+		uintptr_t gap_end = (it != g_pinned.end() && it->first < b) ? it->first : b;
+		/* try the whole 2 MiB-aligned surroundings first (a big buffer then takes few registrations), clipped to
+		 * the neighbours; fall back to exactly the pages asked for (the surroundings may not be mapped, or may
+		 * overlap someone else's registration, which would leave part of them unpinned) */
+		uintptr_t lo = a & ~(big - 1), hi = (gap_end + big - 1) & ~(big - 1);
+		if (it != g_pinned.begin() && std::prev(it)->second > lo) lo = std::prev(it)->second;
+		if (it != g_pinned.end() && it->first < hi) hi = it->first;
+		if (!(lo == a && hi == gap_end) && pin_range(lo, hi) == PIN_NEW) {
+			g_pinned[lo] = hi;
+		} else {
+			const PinResult r = pin_range(a, gap_end);
+			if (r == PIN_FAIL) return -EFAULT;
+			if (r == PIN_NEW) g_pinned[a] = gap_end;
+			hi = gap_end;
+		}
+		a = hi;
+	}
+	return 0;
 }
 
 extern "C" int oimgpu_mem_ensure(const void *addr, size_t len)
@@ -86,33 +134,7 @@ extern "C" int oimgpu_mem_ensure(const void *addr, size_t len)
 		if (cudaPointerGetAttributes(&last, (const uint8_t *)addr + len - 1) == cudaSuccess && last.type != cudaMemoryTypeUnregistered) return 0;
 	}
 	(void)cudaGetLastError();
-	const uintptr_t page = 4096, big = 2u << 20;
-	uintptr_t a = (uintptr_t)addr & ~(page - 1), b = ((uintptr_t)addr + len + page - 1) & ~(page - 1);
-	std::lock_guard<std::mutex> lk(g_pin_mu);
-	/* walk the gaps between what is already pinned */
-	while (a < b) {
-		auto it = g_pinned.upper_bound(a);
-		if (it != g_pinned.begin()) {
-			auto pv = std::prev(it);
-			if (pv->second > a) { a = pv->second; continue; }	/* inside a pinned range: skip it */
-		}
-		uintptr_t gap_end = (it != g_pinned.end() && it->first < b) ? it->first : b;
-		/* try the whole 2 MiB-aligned surroundings first (a big buffer then takes few registrations), clipped to
-		 * the neighbours; fall back to exactly the pages asked for (the surroundings may not be mapped) */
-		uintptr_t lo = a & ~(big - 1), hi = (gap_end + big - 1) & ~(big - 1);
-		if (it != g_pinned.begin() && std::prev(it)->second > lo) lo = std::prev(it)->second;
-		if (it != g_pinned.end() && it->first < hi) hi = it->first;
-		if (!(lo == a && hi == gap_end) && pin_range(lo, hi)) {
-			g_pinned[lo] = hi;
-		} else if (pin_range(a, gap_end)) {
-			g_pinned[a] = gap_end;
-			lo = a; hi = gap_end;
-		} else {
-			return -EFAULT;
-		}
-		a = hi;
-	}
-	return 0;
+	return pin_host_pages(addr, len);
 }
 
 struct oimgpu_copy_chan {

@@ -120,6 +120,8 @@ void refresh_ctrlr_sessions_locked(const std::string &ctrlr);
 cudaError_t launch_copy(cudaStream_t st, int sm_count, void *dst, const void *src, uint64_t nbytes);
 cudaError_t launch_fill(cudaStream_t st, int sm_count, void *dst, uint8_t fill, uint64_t nbytes);
 void unpin_all_host_ranges();	/* oimgpu_mem_ensure's registrations */
+bool host_range_pinned(const void *addr, size_t len);	/* inside one range the library pinned or registered (no driver call) */
+int pin_host_pages(const void *addr, size_t len);	/* pin what of the pages is not pinned yet; -EFAULT */
 
 }  // namespace oimgpu
 

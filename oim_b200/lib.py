@@ -123,6 +123,11 @@ SYMBOLS = [
     ("oimgpu_copy_chan_poll", _I, [_VP, C.POINTER(_VP), _I]),
     ("oimgpu_copy_chan_launches", C.c_ulonglong, [_VP]),
     ("oimgpu_mem_ensure", _I, [_VP, C.c_size_t]),
+    ("oimgpu_bio_chan_open", _I, [C.c_char_p, C.POINTER(_VP)]),
+    ("oimgpu_bio_chan_submit", _I, [_VP, _VP, _U32, _VP, _U32]),
+    ("oimgpu_bio_chan_poll", _I, [_VP, _VP, _I]),
+    ("oimgpu_bio_chan_close", _I, [_VP]),
+    ("oimgpu_bio_chan_launches", C.c_ulonglong, [_VP]),
     ("oimgpu_copy_submit", _I, [_VP, _VP, _VP, _U64]),
     ("oimgpu_fill_submit", _I, [_VP, _VP, C.c_uint8, _U64]),
 ]
@@ -496,3 +501,47 @@ class Lun:
 
     def fill(self, dst: int, value: int, nbytes: int) -> None:
         _chk(load().oimgpu_fill_submit(self.h, dst, value, nbytes), "fill_submit")
+
+
+class BioChan:
+    """Block-I/O channel on one bdev (oimgpu_bio_chan): batches of abi.bio_dtype with an abi.iov_dtype table,
+    completions (abi.bio_cpl_dtype) in submission order."""
+
+    def __init__(self, bdev: str):
+        self.h = C.c_void_p()
+        _chk(load().oimgpu_bio_chan_open(_b(bdev), C.byref(self.h)), "bio_chan_open")
+
+    def close(self):
+        if self.h:
+            load().oimgpu_bio_chan_close(self.h)
+            self.h = C.c_void_p()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
+
+    @property
+    def launches(self) -> int:
+        return load().oimgpu_bio_chan_launches(self.h)
+
+    def submit(self, bios: np.ndarray, iovs: np.ndarray) -> None:
+        assert bios.dtype == abi.bio_dtype and iovs.dtype == abi.iov_dtype
+        bios, iovs = np.ascontiguousarray(bios), np.ascontiguousarray(iovs)
+        _chk(load().oimgpu_bio_chan_submit(self.h, bios.ctypes.data, len(bios), iovs.ctypes.data, len(iovs)),
+             "bio_chan_submit")
+
+    def poll(self, max_n: int) -> np.ndarray:
+        out = np.zeros(max(max_n, 1), dtype=abi.bio_cpl_dtype)
+        n = _chk(load().oimgpu_bio_chan_poll(self.h, out.ctypes.data, max_n), "bio_chan_poll")
+        return out[:n]
+
+    def wait(self, n: int) -> np.ndarray:
+        """reap exactly n completions (blocking: spins on poll)"""
+        got = []
+        while n > 0:
+            c = self.poll(n)
+            got.append(c)
+            n -= len(c)
+        return np.concatenate(got) if got else np.zeros(0, dtype=abi.bio_cpl_dtype)
