@@ -380,8 +380,9 @@ int oimgpu_copy_chan_fill(oimgpu_copy_chan *chan, void *dst, uint8_t fill, uint6
 /* completed operations in submission order: their tags; returns how many (<= max), 0 if none yet */
 int oimgpu_copy_chan_poll(oimgpu_copy_chan *chan, void **tags, int max);
 unsigned long long oimgpu_copy_chan_launches(const oimgpu_copy_chan *chan);	/* kernels launched so far */
-/* make [addr, addr+len) of ordinary host memory accessible to the GPUs (page-granular, idempotent, already
- * registered parts are skipped); -EFAULT if the range cannot be pinned */
+/* make [addr, addr+len) accessible to the GPUs: device memory is taken as it is; host memory is pinned page-granular
+ * and idempotently, and pages already registered (by this library or by another owner) are skipped, so a range that
+ * straddles another owner's buffer has every page mapped; -EFAULT if the range cannot be pinned */
 int oimgpu_mem_ensure(const void *addr, size_t len);
 
 /* ---- block-I/O channel (one level above the copy engine: struct spdk_bdev_fn_table) ---------------------

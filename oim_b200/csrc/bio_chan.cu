@@ -123,20 +123,6 @@ extern "C" int oimgpu_bio_chan_close(oimgpu_bio_chan *c)
 	return 0;
 }
 
-/* a client range the GPU can reach.  Host ranges the library pinned or registered are found without asking the
- * driver.  Otherwise device memory is taken as it is, and host memory is pinned page by page: the shortcut of
- * oimgpu_mem_ensure (both ends known to CUDA) would pass a range whose middle pages were never pinned. */
-static int client_ready(const oimgpu_iov &v, uint32_t take)
-{
-	const void *p = (const void *)(uintptr_t)v.addr;
-	if (host_range_pinned(p, take)) return 0;
-	cudaPointerAttributes attr{};
-	if (cudaPointerGetAttributes(&attr, p) == cudaSuccess &&
-	    (attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged)) return 0;
-	(void)cudaGetLastError();
-	return pin_host_pages(p, take);
-}
-
 /* validate one bio (bdev_malloc_check_iov_len, bdev.c's range check) and emit its segments; 0 or -errno */
 static int emit_bio(oimgpu_bio_chan *c, const oimgpu_bio &b, const oimgpu_iov *iovs, uint32_t niovs)
 {
@@ -160,7 +146,7 @@ static int emit_bio(oimgpu_bio_chan *c, const oimgpu_bio &b, const oimgpu_iov *i
 	uint64_t left = bytes;
 	for (uint32_t i = 0; i < b.iovcnt && left; i++) {
 		const uint32_t take = (uint32_t)std::min<uint64_t>(v[i].len, left);
-		if (take && client_ready(v[i], take) != 0) return -EFAULT;
+		if (take && oimgpu_mem_ensure((const void *)(uintptr_t)v[i].addr, take) != 0) return -EFAULT;
 		left -= take;
 	}
 	left = bytes;

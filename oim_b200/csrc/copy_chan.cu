@@ -80,15 +80,42 @@ bool oimgpu::host_range_pinned(const void *addr, size_t len)
 	return it != g.registered.begin() && (uintptr_t)std::prev(it)->first + std::prev(it)->second >= a + len;
 }
 
-enum PinResult { PIN_NEW, PIN_FOREIGN, PIN_FAIL };
-
-static PinResult pin_range(uintptr_t a, uintptr_t b)
+static bool pin_range(uintptr_t a, uintptr_t b)
 {
-	cudaError_t e = cudaHostRegister((void *)a, b - a, cudaHostRegisterMapped | cudaHostRegisterPortable);
-	if (e == cudaSuccess) return PIN_NEW;
+	if (cudaHostRegister((void *)a, b - a, cudaHostRegisterMapped | cudaHostRegisterPortable) == cudaSuccess) return true;
 	(void)cudaGetLastError();
-	/* registered by someone else (cudaHostAlloc, oimgpu_mem_register) - theirs to keep or let go */
-	return e == cudaErrorHostMemoryAlreadyRegistered ? PIN_FOREIGN : PIN_FAIL;
+	return false;
+}
+
+/* a page CUDA already knows at its first or its last byte: registered or allocated pinned by another owner
+ * (oimgpu_mem_register, cudaHostRegister, cudaHostAlloc) - theirs to keep or let go */
+static bool foreign_page(uintptr_t p)
+{
+	for (uintptr_t q : {p, p + 4095}) {
+		cudaPointerAttributes attr{};
+		if (cudaPointerGetAttributes(&attr, (const void *)q) == cudaSuccess && attr.type != cudaMemoryTypeUnregistered) return true;
+		(void)cudaGetLastError();
+	}
+	return false;
+}
+
+/* [a, b) could not be registered as a whole: pin each maximal run of its pages that no other owner holds.  Rare (a
+ * range in, or straddling the edge of, another owner's buffer), so two driver queries per page are fine.  A run
+ * that still fails - unmapped, or sharing a page with a registration that touches neither end of it - is refused,
+ * never taken as pinned. */
+static int pin_around_foreign(uintptr_t a, uintptr_t b)
+{
+	const uintptr_t page = 4096;
+	while (a < b) {
+		while (a < b && foreign_page(a)) a += page;
+		uintptr_t e = a;
+		while (e < b && !foreign_page(e)) e += page;
+		if (e == a) break;
+		if (!pin_range(a, e)) return -EFAULT;
+		g_pinned[a] = e;
+		a = e;
+	}
+	return 0;
 }
 
 int oimgpu::pin_host_pages(const void *addr, size_t len)
@@ -106,16 +133,16 @@ int oimgpu::pin_host_pages(const void *addr, size_t len)
 		uintptr_t gap_end = (it != g_pinned.end() && it->first < b) ? it->first : b;
 		/* try the whole 2 MiB-aligned surroundings first (a big buffer then takes few registrations), clipped to
 		 * the neighbours; fall back to exactly the pages asked for (the surroundings may not be mapped, or may
-		 * overlap someone else's registration, which would leave part of them unpinned) */
+		 * overlap someone else's registration, which would leave part of them unpinned).  Where the exact pages
+		 * cannot be registered either, they are taken page by page. */
 		uintptr_t lo = a & ~(big - 1), hi = (gap_end + big - 1) & ~(big - 1);
 		if (it != g_pinned.begin() && std::prev(it)->second > lo) lo = std::prev(it)->second;
 		if (it != g_pinned.end() && it->first < hi) hi = it->first;
-		if (!(lo == a && hi == gap_end) && pin_range(lo, hi) == PIN_NEW) {
+		if (!(lo == a && hi == gap_end) && pin_range(lo, hi)) {
 			g_pinned[lo] = hi;
 		} else {
-			const PinResult r = pin_range(a, gap_end);
-			if (r == PIN_FAIL) return -EFAULT;
-			if (r == PIN_NEW) g_pinned[a] = gap_end;
+			if (pin_range(a, gap_end)) g_pinned[a] = gap_end;
+			else if (pin_around_foreign(a, gap_end) != 0) return -EFAULT;
 			hi = gap_end;
 		}
 		a = hi;
@@ -127,12 +154,13 @@ extern "C" int oimgpu_mem_ensure(const void *addr, size_t len)
 {
 	if (!g.inited || g.control_only) return -ENODEV;
 	if (!addr || !len) return 0;
+	/* host ranges the library pinned or registered are found without asking the driver.  Otherwise device memory
+	 * is taken as it is, and host memory is pinned page by page: a range whose two ends CUDA knows may still have
+	 * pages in between that nobody pinned. */
+	if (host_range_pinned(addr, len)) return 0;
 	cudaPointerAttributes attr{};
-	if (cudaPointerGetAttributes(&attr, addr) == cudaSuccess && attr.type != cudaMemoryTypeUnregistered) {
-		/* device memory, or host memory CUDA already knows: check the far end too (a range may straddle) */
-		cudaPointerAttributes last{};
-		if (cudaPointerGetAttributes(&last, (const uint8_t *)addr + len - 1) == cudaSuccess && last.type != cudaMemoryTypeUnregistered) return 0;
-	}
+	if (cudaPointerGetAttributes(&attr, addr) == cudaSuccess &&
+	    (attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged)) return 0;
 	(void)cudaGetLastError();
 	return pin_host_pages(addr, len);
 }
