@@ -126,12 +126,14 @@ static int refresh_peers_locked(oimgpu_lun *L)
 	for (int t = 0; t < OIMGPU_CTRLR_MAX_DEVS; t++) {
 		if (!L->peer_bdev[t].empty() && g.bdevs[L->peer_bdev[t]]->stores.size() > 1) L->any_mirror = true;
 	}
+	/* a launch still in flight finishes with the peers it started with: published under it, a mirror attached
+	 * while the plain kernel runs would be served by a kernel that ignores Segment::mirror (GOOD, replica 0 only) */
+	if (!L->poller_active) CU_OK(cudaStreamSynchronize(L->stream));
 	/* publish the pointers after the contexts they point at (same stream); a separate stream so that a
 	 * resident poller kernel on L->stream does not block the update */
 	CU_OK(cudaMemcpyAsync((uint8_t *)L->d_ctx + offsetof(LunCtx, peer), L->h_ctx.peer, sizeof(L->h_ctx.peer),
 			      cudaMemcpyHostToDevice, L->copy_stream));
 	CU_OK(cudaStreamSynchronize(L->copy_stream));
-	if (!L->poller_active) CU_OK(cudaStreamSynchronize(L->stream));
 	if (restart && was_polling) {
 		int rc = oimgpu_lun_start_poller(L, L->poller_max_ctas, L->poller_idle_ms);
 		if (rc < 0) return rc;

@@ -66,19 +66,28 @@ def test_multi_target_restatement_matches_reference(oracles, seed, kind):
 
 
 class Controller:
-    """three Malloc bdevs on one controller, as MapVolume x3 leaves them.  sizes: {target: (blocks, block size)}"""
+    """three Malloc bdevs on one controller, as MapVolume x3 leaves them.  sizes: {target: (blocks, block size)};
+    mirrors: {target: devices} makes that target a mirrored bdev with a replica on each device (all replicas start
+    with the same contents)"""
 
-    def __init__(self, gpu, only=None, sizes=None):
+    def __init__(self, gpu, only=None, sizes=None, mirrors=None):
         self.gpu = gpu
         self.sizes = sizes or {t: (TARGETS[t], 512) for t in TARGETS}
+        self.mirrors = dict(mirrors or {})
         tag = next(_seq)
         self.ctrlr = f"mtc{tag}"
         self.names = {t: f"mtb{tag}_{t}" for t in TARGETS}
         gpu.construct_vhost_scsi_controller(self.ctrlr)
         self.attached = set()
         for t, (nb, bs) in self.sizes.items():
-            gpu.construct_malloc_bdev(nb, bs, name=self.names[t], device=0)
-            gpu.bdev_write_raw(self.names[t], 0, traces.pattern_bytes(7 + (t if t != 1 else 0), 0, nb * bs))
+            if t in self.mirrors:
+                gpu.construct_mirror_bdev(nb, bs, self.mirrors[t], name=self.names[t])
+                assert gpu.get_bdevs(self.names[t])[0]["replicas"] == len(self.mirrors[t])
+            else:
+                gpu.construct_malloc_bdev(nb, bs, name=self.names[t], device=0)
+            init = traces.pattern_bytes(7 + (t if t != 1 else 0), 0, nb * bs)
+            for rep in range(self.replicas(t)):
+                gpu.bdev_write_raw(self.names[t], 0, init, replica=rep)
             if only is None or t in only:
                 self.attach(t)
 
@@ -93,8 +102,16 @@ class Controller:
     def ids(self):
         return {x["scsi_dev_num"]: x["id"] for x in self.gpu.get_vhost_controllers(self.ctrlr)[0]["backend_specific"]["scsi"]}
 
+    def replicas(self, t):
+        return len(self.mirrors.get(t, [0]))
+
     def stores(self):
         return {t: self.gpu.bdev_read_raw(self.names[t], 0, nb * bs) for t, (nb, bs) in self.sizes.items()}
+
+    def replica_stores(self):
+        """{(target, replica): store} over every replica of every target"""
+        return {(t, r): self.gpu.bdev_read_raw(self.names[t], 0, nb * bs, replica=r)
+                for t, (nb, bs) in self.sizes.items() for r in range(self.replicas(t))}
 
     def close(self):
         for t in list(self.attached):

@@ -213,16 +213,32 @@ def test_nbd_restatement_matches_reference(oracles, seed):
 @pytest.mark.gpu
 @pytest.mark.parametrize("seed", range(4))
 def test_cuda_nbd_matches_reference(gpu, oracles, seed):
+    _cuda_nbd(gpu, oracles, seed, f"nbd{seed}", 1)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("seed", range(4))
+def test_cuda_nbd_on_a_mirror_matches_reference(gpu, oracles, seed):
+    """the same scripts on a mirror of three replicas on cuda:0: WRITE and TRIM reach every replica, READ answers from
+    replica 0, and the counters count each I/O once"""
+    _cuda_nbd(gpu, oracles, seed, f"nbdm{seed}", 3)
+
+
+def _cuda_nbd(gpu, oracles, seed, name, replicas):
     ops = script(seed)
     tail = tails()["disc" if seed % 2 == 0 else "garbage"]
     if oracles.ref_available():
         want, want_store = run_reference(oracles, ops, tail)
     else:
         want, want_store, _ = run_restatement(oracles, ops, tail)
-    name = f"nbd{seed}"
-    gpu.construct_malloc_bdev(NB, BS, name=name, device=0)
+    if replicas > 1:
+        gpu.construct_mirror_bdev(NB, BS, [0] * replicas, name=name)
+        assert gpu.get_bdevs(name)[0]["replicas"] == replicas
+    else:
+        gpu.construct_malloc_bdev(NB, BS, name=name, device=0)
     try:
-        gpu.bdev_write_raw(name, 0, traces.pattern_bytes(7, 0, NB * BS))
+        for r in range(replicas):
+            gpu.bdev_write_raw(name, 0, traces.pattern_bytes(7, 0, NB * BS), replica=r)
         a, b = socket.socketpair()
         a.settimeout(20)
         rc = []
@@ -239,10 +255,15 @@ def test_cuda_nbd_matches_reference(gpu, oracles, seed):
         assert len(got) == len(want)
         for i, (g, w) in enumerate(zip(got, want)):
             assert g == w, f"reply {i} to {ops[i][:3] if i < len(ops) else 'tail'} differs: {g[:24]!r} vs {w[:24]!r}"
-        assert (gpu.bdev_read_raw(name, 0, NB * BS) == want_store).all()
+        for r in range(replicas):
+            bad = np.nonzero(gpu.bdev_read_raw(name, 0, NB * BS, replica=r) != want_store)[0]
+            assert not len(bad), f"replica {r} of {replicas} differs from the reference's store at {len(bad)} bytes, first {bad[:8]}"
         st = gpu.get_bdevs_iostat(name)
         ok_reads = sum(1 for op, r in zip(ops, want) if op[0] == READ and r[4:8] == b"\x00" * 4)
         ok_writes = sum(1 for op, r in zip(ops, want) if op[0] == WRITE and r[4:8] == b"\x00" * 4)
         assert (st["num_read_ops"], st["num_write_ops"]) == (ok_reads, ok_writes)
+        ok_trims = [op for op, r in zip(ops, want) if op[0] == TRIM and r[4:8] == b"\x00" * 4]
+        assert (st["num_unmap_ops"], st["bytes_unmapped"]) == (len(ok_trims), sum(op[2] for op in ok_trims))
+        assert st["bytes_written"] == sum(op[2] for op, r in zip(ops, want) if op[0] == WRITE and r[4:8] == b"\x00" * 4)
     finally:
         gpu.delete_bdev(name)

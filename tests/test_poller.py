@@ -7,7 +7,7 @@ import pytest
 
 import util
 from oim_b200 import abi, traces, vring
-from test_vring import VQ_KERNELS
+from test_vring import VQ_KERNELS, VQ_MIRROR_KERNELS
 
 pytestmark = pytest.mark.gpu
 WATCHDOG_MS = 4000
@@ -15,13 +15,32 @@ WATCHDOG_MS = 4000
 # OIMGPU_NO_SHARED_QUEUES=1 oim_lun_vring_kernel, where mover warp 0 publishes; with OIMGPU_NO_VRING_KERNEL=1 as well,
 # oim_lun_queue_kernel, where the parser publishes
 POLLER_VARIANTS = VQ_KERNELS
+# the two mirror kernels resident, on two and three replicas on cuda:0: variant -> (environment, replicas)
+MIRROR_POLLER_VARIANTS = {f"{k}-r{r}": (env, r) for r in (2, 3) for k, env in VQ_MIRROR_KERNELS.items()}
+POLLER_CASES = {**{k: (env, 1) for k, env in POLLER_VARIANTS.items()}, **MIRROR_POLLER_VARIANTS}
 
 
-def _setup(gpu, name, nb):
-    gpu.construct_malloc_bdev(nb, 512, name=name, device=0)
+def _shared(variant: str) -> bool:
+    """whether the variant's resident kernel shares the queues a pass at a time (shared_launches)"""
+    return variant == "shared" or variant.startswith("mirror-shared")
+
+
+def _setup(gpu, name, nb, replicas=1):
+    if replicas > 1:
+        gpu.construct_mirror_bdev(nb, 512, [0] * replicas, name=name)
+        assert gpu.get_bdevs(name)[0]["replicas"] == replicas
+    else:
+        gpu.construct_malloc_bdev(nb, 512, name=name, device=0)
     gpu.construct_vhost_scsi_controller(name + ".ctl")
     gpu.add_vhost_scsi_lun(name + ".ctl", 0, name)
-    gpu.bdev_write_raw(name, 0, traces.pattern_bytes(7, 0, nb * 512))
+    for r in range(replicas):
+        gpu.bdev_write_raw(name, 0, traces.pattern_bytes(7, 0, nb * 512), replica=r)
+
+
+def _check_replicas(gpu, name, nb, replicas, want_store):
+    for r in range(replicas):
+        bad = np.nonzero(gpu.bdev_read_raw(name, 0, nb * 512, replica=r) != want_store)[0]
+        assert not len(bad), f"replica {r} of {replicas} differs from the oracle at {len(bad)} bytes, first {bad[:8]}"
 
 
 def _teardown(gpu, name):
@@ -33,6 +52,18 @@ def _teardown(gpu, name):
 @pytest.mark.timeout(120)
 def test_poller_serves_ring_doorbells(gpu, oracles):
     """closed loop, qd=32 per queue: submit 32, ring the doorbell, wait for the completion counter"""
+    _ring_doorbells(gpu, oracles, "pl0", {}, 1, 64)
+
+
+@pytest.mark.timeout(120)
+@pytest.mark.parametrize("variant", list(MIRROR_POLLER_VARIANTS))
+def test_poller_serves_ring_doorbells_on_a_mirror(gpu, oracles, variant):
+    """the same on a mirror, with rings of 256 so that the resident mirror-shared kernel has CTAs to share them"""
+    env, replicas = MIRROR_POLLER_VARIANTS[variant]
+    _ring_doorbells(gpu, oracles, f"plm{variant}", env, replicas, 256, shared=_shared(variant))
+
+
+def _ring_doorbells(gpu, oracles, name, env, replicas, queue_size, shared=None):
     import torch
     nb, nq, rounds = 1 << 16, 4, 12
     t = traces.partitioned_queues(nq, 32 * rounds, nb, pattern="randrw", read_pct=60, io_blocks=8)
@@ -43,14 +74,16 @@ def test_poller_serves_ring_doorbells(gpu, oracles):
         oa = host.copy()
         want = o.submit(t.reqs, t.bind(oa.ctypes.data))
         want_store = o.store.copy()
-    _setup(gpu, "pl0", nb)
+    _setup(gpu, name, nb, replicas)
     try:
         arena = torch.from_numpy(host.copy()).pin_memory()
         iovs = t.bind(arena.data_ptr())
         per_q = 32 * rounds
         got = np.zeros(len(t.reqs), dtype=abi.cpl_dtype)
-        with gpu.Lun("pl0.ctl", 0, num_queues=nq, queue_size=64) as lun:
+        with util.environ(**env), gpu.Lun(name + ".ctl", 0, num_queues=nq, queue_size=queue_size) as lun:
             assert lun.start_poller(idle_timeout_ms=WATCHDOG_MS) >= nq      # workers: one per queue, more when they share queues
+            if shared is not None:
+                assert lun.shared_launches == shared, f"the resident kernel {'does not share' if shared else 'shares'} the queues"
             launches_before = None
             try:
                 for r in range(rounds):
@@ -72,9 +105,9 @@ def test_poller_serves_ring_doorbells(gpu, oracles):
         assert stats["kernel_launches"] == 1, "one resident kernel served every round"
         util.assert_cpls_equal(got, want, t.reqs)
         assert (arena.numpy() == oa).all()
-        assert (gpu.bdev_read_raw("pl0", 0, nb * 512) == want_store).all()
+        _check_replicas(gpu, name, nb, replicas, want_store)
     finally:
-        _teardown(gpu, "pl0")
+        _teardown(gpu, name)
 
 
 @pytest.mark.timeout(120)
@@ -276,7 +309,7 @@ def _wait_used(used_idx, target, what, timeout_s=20.0):
 
 
 @pytest.mark.timeout(180)
-@pytest.mark.parametrize("variant", list(POLLER_VARIANTS))
+@pytest.mark.parametrize("variant", list(POLLER_CASES))
 def test_poller_guest_ring_across_the_index_wrap(gpu, oracles, variant):
     """test_poller_guest_reuses_ring_and_buffers from cursor 65536 - 100: rounds of 40 requests carry avail->idx and
     used->idx across the 16-bit wrap and the ring's end under the resident kernel.  After stop_poller the cursors
@@ -305,7 +338,8 @@ def test_poller_guest_ring_across_the_index_wrap(gpu, oracles, variant):
         want_cursors = (la, lu)
     assert want_cursors == ((start + rounds * per) & 0xFFFF,) * 2
     name = f"pvw{variant}"
-    _setup(gpu, name, nb)
+    env, replicas = POLLER_CASES[variant]
+    _setup(gpu, name, nb, replicas)
     try:
         img0 = imgs[0]
         guest = torch.from_numpy(img0.arena.copy()).pin_memory()
@@ -315,13 +349,13 @@ def test_poller_guest_ring_across_the_index_wrap(gpu, oracles, variant):
         avail_idx[0] = start                                   # nothing published yet
         base = guest.data_ptr()
         lo, hi = img0.avail_off, img0.used_off + 4 + 8 * R
-        with util.environ(**POLLER_VARIANTS[variant]), gpu.Lun(f"{name}.ctl", 0, num_queues=1, queue_size=32) as lun:
+        with util.environ(**env), gpu.Lun(f"{name}.ctl", 0, num_queues=1, queue_size=32) as lun:
             lun.set_mem_table(img0.region_table(base))
             lun.vq_attach(0, base + img0.desc_off, base + img0.avail_off, base + img0.used_off, R, start, start)
             shared = lun.shared_launches
             lun.start_poller(idle_timeout_ms=WATCHDOG_MS)
             try:
-                assert lun.shared_launches - shared == (variant == "shared"), f"the poller is not the {variant} kernel"
+                assert lun.shared_launches - shared == _shared(variant), f"the poller is not the {variant} kernel"
                 for r in range(rounds):
                     img, (la, lu) = imgs[r], cur[r]
                     if r:
@@ -345,7 +379,8 @@ def test_poller_guest_ring_across_the_index_wrap(gpu, oracles, variant):
             finally:
                 lun.stop_poller()
             assert lun.vq_detach(0) == want_cursors
-        assert (gpu.bdev_read_raw(name, 0, nb * 512) == want_store).all()
+            assert lun.iostat()["kernel_launches"] == 1, "one resident kernel served every round"
+        _check_replicas(gpu, name, nb, replicas, want_store)
     finally:
         _teardown(gpu, name)
 
@@ -357,7 +392,7 @@ def _spin_us(us: float) -> None:
 
 
 @pytest.mark.timeout(180)
-@pytest.mark.parametrize("variant", list(POLLER_VARIANTS))
+@pytest.mark.parametrize("variant", list(POLLER_CASES))
 def test_poller_guest_publishes_while_a_batch_moves(gpu, oracles, variant):
     """A Linux guest bumps avail->idx for every request it adds, so the resident kernel finds new requests on a ring
     while the batch before them is still moving.  First 32 READs of 1 MiB into guest memory (pinned host memory:
@@ -390,7 +425,8 @@ def test_poller_guest_publishes_while_a_batch_moves(gpu, oracles, variant):
         assert o.vq_process(ref, start, start) == (n, end, end)
         want_store = o.store.copy()
     name = f"pvs{variant}"
-    _setup(gpu, name, nb)
+    env, replicas = POLLER_CASES[variant]
+    _setup(gpu, name, nb, replicas)
     try:
         guest = torch.from_numpy(img.arena.copy()).pin_memory()
         g = guest.numpy()
@@ -401,13 +437,13 @@ def test_poller_guest_publishes_while_a_batch_moves(gpu, oracles, variant):
         ring[pos[32:]] = (ring[pos[32:]] + 1) % R             # not yet written by the guest: wrong heads
         avail_idx[0] = start
         base = guest.data_ptr()
-        with util.environ(**POLLER_VARIANTS[variant]), gpu.Lun(f"{name}.ctl", 0, num_queues=1, queue_size=32) as lun:
+        with util.environ(**env), gpu.Lun(f"{name}.ctl", 0, num_queues=1, queue_size=32) as lun:
             lun.set_mem_table(img.region_table(base))
             lun.vq_attach(0, base + img.desc_off, base + img.avail_off, base + img.used_off, R, start, start)
             shared = lun.shared_launches
             lun.start_poller(idle_timeout_ms=WATCHDOG_MS)
             try:
-                assert lun.shared_launches - shared == (variant == "shared"), f"the poller is not the {variant} kernel"
+                assert lun.shared_launches - shared == _shared(variant), f"the poller is not the {variant} kernel"
                 avail_idx[0] = (start + 32) & 0xFFFF               # the 32 large READs
                 for k in range(32, n):
                     _spin_us(30)
@@ -417,6 +453,7 @@ def test_poller_guest_publishes_while_a_batch_moves(gpu, oracles, variant):
             finally:
                 lun.stop_poller()
             cursors = lun.vq_detach(0)
+            assert lun.iostat()["kernel_launches"] == 1, "one resident kernel served the whole stream"
         used = img.used_in_order(g, start, n)
         assert [int(i) for i in used["id"]] == img.heads, "used elements out of ring order"
         assert sorted((int(i), int(l)) for i, l in used) == sorted((int(i), int(l)) for i, l in ref.used_in_order(None, start, n))
@@ -424,6 +461,6 @@ def test_poller_guest_publishes_while_a_batch_moves(gpu, oracles, variant):
         got, want = img.masked(g.copy()), ref.masked(ref.arena)
         assert (got == want).all(), f"guest memory differs at {np.nonzero(got != want)[0][:8]}"
         assert cursors == (end, end)
-        assert (gpu.bdev_read_raw(name, 0, nb * 512) == want_store).all()
+        _check_replicas(gpu, name, nb, replicas, want_store)
     finally:
         _teardown(gpu, name)

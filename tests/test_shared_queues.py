@@ -22,15 +22,25 @@ def _oracle(oracles, t, nb, seed=7):
     return cpls, arena, store
 
 
-def _run_batch(gpu, name, t, nb, nq, per_q, seed=7, kernel="shared"):
+def _make_bdev(gpu, name, nb, replicas):
+    if replicas > 1:
+        gpu.construct_mirror_bdev(nb, 512, [0] * replicas, name=name)
+        assert gpu.get_bdevs(name)[0]["replicas"] == replicas
+    else:
+        gpu.construct_malloc_bdev(nb, 512, name=name, device=0)
+
+
+def _run_batch(gpu, name, t, nb, nq, per_q, seed=7, kernel="shared", replicas=1):
     """one oimgpu_submit_batch launch: queue q <- requests [q*per_q, (q+1)*per_q), everything in HBM.
-    kernel="exclusive": with OIMGPU_NO_SHARED_QUEUES=1 (one CTA per queue)"""
+    kernel="exclusive": with OIMGPU_NO_SHARED_QUEUES=1 (one CTA per queue).  replicas > 1: on a mirror with that
+    many replicas on cuda:0; every replica must end up equal to replica 0, whose store is returned"""
     import torch
-    gpu.construct_malloc_bdev(nb, 512, name=name, device=0)
+    _make_bdev(gpu, name, nb, replicas)
     gpu.construct_vhost_scsi_controller(name + ".ctl")
     gpu.add_vhost_scsi_lun(name + ".ctl", 0, name)
     try:
-        gpu.bdev_write_raw(name, 0, traces.pattern_bytes(seed, 0, nb * 512))
+        for r in range(replicas):
+            gpu.bdev_write_raw(name, 0, traces.pattern_bytes(seed, 0, nb * 512), replica=r)
         host = np.zeros(t.arena_bytes, dtype=np.uint8)
         traces.fill_arena(host, t)
         dev = torch.from_numpy(host).to("cuda:0")
@@ -45,7 +55,11 @@ def _run_batch(gpu, name, t, nb, nq, per_q, seed=7, kernel="shared"):
             stats = lun.iostat()
         assert stats["kernel_launches"] == 1
         cpls = np.frombuffer(d_cpls.cpu().numpy().tobytes(), dtype=abi.cpl_dtype)
-        return cpls, dev.cpu().numpy(), gpu.bdev_read_raw(name, 0, nb * 512), shared, stats
+        store = gpu.bdev_read_raw(name, 0, nb * 512)
+        for r in range(1, replicas):
+            bad = np.nonzero(gpu.bdev_read_raw(name, 0, nb * 512, replica=r) != store)[0]
+            assert not len(bad), f"replica {r} of {replicas} differs from replica 0 at {len(bad)} bytes, first {bad[:8]}"
+        return cpls, dev.cpu().numpy(), store, shared, stats
     finally:
         gpu.remove_vhost_scsi_target(name + ".ctl", 0)
         gpu.remove_vhost_controller(name + ".ctl")
@@ -56,6 +70,18 @@ def _run_batch(gpu, name, t, nb, nq, per_q, seed=7, kernel="shared"):
 def test_shared_queues_match_sequential_result(gpu, oracles, nq, per_q, read_pct):
     """few deep queues, each hammering a SMALL LBA window (every pass collides with its neighbours: RAW, WAW and
     WAR pairs across the CTAs that share the queue)"""
+    _shared_queues(gpu, oracles, nq, per_q, read_pct, 1)
+
+
+@pytest.mark.parametrize("replicas", [2, 3])
+@pytest.mark.parametrize("nq,per_q,read_pct", [(3, 4096, 50), (7, 2048, 70)])
+def test_shared_queues_on_a_mirror_match_sequential_result(gpu, oracles, nq, per_q, read_pct, replicas):
+    """the same on a mirror: the shared mirror kernel's cross-CTA hazards, with every replica equal to the
+    sequential result"""
+    _shared_queues(gpu, oracles, nq, per_q, read_pct, replicas)
+
+
+def _shared_queues(gpu, oracles, nq, per_q, read_pct, replicas):
     window = 4096                                   # blocks per queue: 512 distinct 4 KiB slots for thousands of requests
     nb = max(1 << 16, nq * window)
     parts = [traces.uniform_trace(per_q, nb, io_blocks=8, pattern="randrw", read_pct=read_pct, lba_lo=q * window,
@@ -70,7 +96,7 @@ def test_shared_queues_match_sequential_result(gpu, oracles, nq, per_q, read_pct
         iovs["addr"][sl] += np.uint64(q * per_q * stride)
     t = traces.Trace(reqs, iovs, nq * per_q * stride, f"shared-{nq}x{per_q}")
     want = _oracle(oracles, t, nb)
-    got = _run_batch(gpu, f"shq{nq}_{read_pct}", t, nb, nq, per_q)
+    got = _run_batch(gpu, f"shq{nq}_{read_pct}_{replicas}", t, nb, nq, per_q, replicas=replicas)
     assert got[3] == 1, "the launch did not take the shared-queue path"
     util.assert_cpls_equal(got[0], want[0], t.reqs)
     assert (got[1] == want[1]).all(), "read payloads differ from the sequential result"
@@ -98,56 +124,83 @@ def test_cross_queue_write_after_write_is_one_of_the_legal_outcomes(gpu):
     """Queues are mutually unordered (as for any multi-queue block device; the reference interleaves them in an order
     that depends on poller timing).  What IS guaranteed: every word of the block is from the LAST write of one of
     the queues, never from an earlier write of a queue that wrote the LBA again."""
+    _cross_queue_waw(gpu, "waw0", 1)
+
+
+@pytest.mark.parametrize("replicas", [2, 3])
+def test_cross_queue_write_after_write_on_a_mirror(gpu, replicas):
+    """The same on a mirror, plus slots that only one queue writes.  Each replica on its own obeys the per-word rule.
+    The replicas may differ from each other in the words two queues wrote at the same time (each replica's stores of
+    two racing warps land in their own order); a slot that one queue alone wrote is the same on every replica."""
+    _cross_queue_waw(gpu, f"wawm{replicas}", replicas, solo=64)
+
+
+def _cross_queue_waw(gpu, name, replicas, solo=0):
+    """every queue writes each of `slots` shared 4 KiB slots `rounds` times in its own random order; slot
+    slots + k (k < solo) is written `rounds` times by queue k % nq only.  Returns nothing: asserts on every replica."""
     import torch
     nb, slots, nq = 1 << 14, 256, 4
     rounds = 8                                      # every queue writes every slot `rounds` times, in its own random order
     rng = np.random.default_rng(5)
-    per_q = slots * rounds
+    per_q = slots * rounds + solo // nq * rounds
     b = abi.Batch(0)
-    last = np.zeros((nq, slots), dtype=np.int64)    # request index of queue q's last write to the slot
+    last = np.zeros((nq, slots + solo), dtype=np.int64)     # request index of queue q's last write to the slot
     off = 0
     for q in range(nq):
-        order = np.concatenate([rng.permutation(slots) for _ in range(rounds)])
+        mine = np.arange(slots + q, slots + solo, nq)
+        order = np.concatenate([rng.permutation(np.concatenate([np.arange(slots), mine])) for _ in range(rounds)])
         for k, sl in enumerate(order):
             i = q * per_q + k
             b.write(int(sl) * 8, 8, [(off, 4096)])
             last[q, sl] = i
             off += 4096
     reqs, iovs = b.arrays()
+    assert len(reqs) == nq * per_q
     t = traces.Trace(reqs, iovs, off, "waw")
     arena = np.zeros(off, dtype=np.uint8)
     arena.view(np.uint64)[:] = np.repeat(np.arange(nq * per_q, dtype=np.uint64), 512) * np.uint64(0x9E3779B97F4A7C15) + np.uint64(1)
-    name = "waw0"
-    gpu.construct_malloc_bdev(nb, 512, name=name, device=0)
-    gpu.construct_vhost_scsi_controller("waw.ctl")
-    gpu.add_vhost_scsi_lun("waw.ctl", 0, name)
+    ctl = name + ".ctl"
+    _make_bdev(gpu, name, nb, replicas)
+    gpu.construct_vhost_scsi_controller(ctl)
+    gpu.add_vhost_scsi_lun(ctl, 0, name)
     try:
         dev = torch.from_numpy(arena).to("cuda:0")
         d_reqs = torch.from_numpy(t.reqs.view(np.uint8).copy()).cuda()
         d_iovs = torch.from_numpy(t.bind(dev.data_ptr()).view(np.uint8).copy()).cuda()
         d_cpls = torch.zeros(len(t.reqs) * 48, dtype=torch.uint8, device="cuda")
         torch.cuda.synchronize()
-        with gpu.Lun("waw.ctl", 0, num_queues=nq, queue_size=32) as lun:
+        with gpu.Lun(ctl, 0, num_queues=nq, queue_size=32) as lun:
             lun.submit_batch(nq, per_q, d_reqs.data_ptr(), d_iovs.data_ptr(), len(t.iovs), d_cpls.data_ptr(), abi.MEM_DEVICE)
             lun.sync()
         c = np.frombuffer(d_cpls.cpu().numpy().tobytes(), dtype=abi.cpl_dtype)
         assert not c["status"].any()
-        store = gpu.bdev_read_raw(name, 0, slots * 4096).view(np.uint64).reshape(slots, 512)
         with np.errstate(over="ignore"):
-            legal = last.astype(np.uint64) * np.uint64(0x9E3779B97F4A7C15) + np.uint64(1)      # [nq, slots]
-        # Two queues writing one block at the same time are two warps storing 16-byte vectors side by side: the block
-        # may end up with vectors of both (the reference, one reactor, would leave one whole request; NVMe promises
-        # no more than this beyond its atomic write unit).  What must hold for EVERY word: it is from the LAST write
-        # of one of the queues.
-        ok = np.zeros(store.shape, dtype=bool)
-        for q in range(nq):
-            ok |= store == legal[q][:, None]
-        assert ok.all(), f"{int((~ok).sum())} words are not from the last write of any queue (an overwritten write survived)"
-        torn = int((store != store[:, :1]).any(axis=1).sum())
-        print(f"cross-queue WAW: {torn} of {slots} blocks hold vectors of more than one queue's last write")
+            legal = last.astype(np.uint64) * np.uint64(0x9E3779B97F4A7C15) + np.uint64(1)      # [nq, slots + solo]
+        stores = [gpu.bdev_read_raw(name, 0, (slots + solo) * 4096, replica=r).view(np.uint64).reshape(slots + solo, 512)
+                  for r in range(replicas)]
+        for r, store in enumerate(stores):
+            shared = store[:slots]
+            # Two queues writing one block at the same time are two warps storing 16-byte vectors side by side: the
+            # block may end up with vectors of both (the reference, one reactor, would leave one whole request; NVMe
+            # promises no more than this beyond its atomic write unit).  What must hold for EVERY word: it is from the
+            # LAST write of one of the queues.
+            ok = np.zeros(shared.shape, dtype=bool)
+            for q in range(nq):
+                ok |= shared == legal[q, :slots][:, None]
+            assert ok.all(), f"replica {r}: {int((~ok).sum())} words are not from the last write of any queue (an overwritten write survived)"
+            for k in range(solo):
+                q = k % nq
+                assert (store[slots + k] == legal[q, slots + k]).all(), f"replica {r}: slot {slots + k}, written by queue {q} alone"
+            torn = int((shared != shared[:, :1]).any(axis=1).sum())
+            print(f"cross-queue WAW, replica {r}: {torn} of {slots} blocks hold vectors of more than one queue's last write")
+        for r in range(1, replicas):
+            differ = stores[r] != stores[0]
+            assert not differ[slots:].any(), f"replica {r}: a slot one queue alone wrote differs from replica 0"
+            print(f"cross-queue WAW: replica {r} differs from replica 0 in {int(differ.sum())} of {slots * 512} words "
+                  f"of the slots the queues share")
     finally:
-        gpu.remove_vhost_scsi_target("waw.ctl", 0)
-        gpu.remove_vhost_controller("waw.ctl")
+        gpu.remove_vhost_scsi_target(ctl, 0)
+        gpu.remove_vhost_controller(ctl)
         gpu.delete_bdev(name)
 
 

@@ -114,7 +114,7 @@ def _run_device_arrays(lun, reqs: np.ndarray, iovs: np.ndarray) -> np.ndarray:
 def run_cuda(lib, trace: traces.Trace, num_blocks: int, *, block_size: int = 512, store_seed: int | None = 7,
              arena_seed: int = 0x5EED, target: int = 0, mem: str = "device", removed: bool = False,
              queue_size: int = 1024, name: str | None = None, kernel: str | None = None, histogram: bool = False,
-             lun_removed: bool = False):
+             lun_removed: bool = False, replicas: int = 2):
     """Same replay through liboimgpu.so on cuda:0.  mem="device": client buffers in HBM (a torch
     tensor); mem="host": client buffers in pinned, registered host memory.
 
@@ -122,7 +122,8 @@ def run_cuda(lib, trace: traces.Trace, num_blocks: int, *, block_size: int = 512
     the library reports that it did (iostat kernel_launches, Lun.shared_launches).  The ring is sized to hold
     the trace (queue_size is then ignored); a trace longer than a ring goes in as device arrays.  One launch
     also keeps the write-mix switch (a write-hot session stops sharing) from changing the variant mid-trace.
-    The mirror variants put two replicas on cuda:0, and check that they end up equal.
+    The mirror variants put `replicas` replicas on cuda:0, write the initial store to each, and check that they all
+    end up equal to replica 0.
 
     histogram: enable the bdev's latency histogram first; stats["histogram_total"] is then its number of tallies.
     lun_removed: the session sees its LUN being torn down (every request aborted)."""
@@ -135,7 +136,7 @@ def run_cuda(lib, trace: traces.Trace, num_blocks: int, *, block_size: int = 512
     tag = next(_seq)
     bname, cname = name or f"par{tag}", f"parctl{tag}"
     if mirror:
-        lib.construct_mirror_bdev(num_blocks, block_size, [0, 0], name=bname)
+        lib.construct_mirror_bdev(num_blocks, block_size, [0] * replicas, name=bname)
     else:
         lib.construct_malloc_bdev(num_blocks, block_size, name=bname, device=0)
     lib.construct_vhost_scsi_controller(cname)
@@ -146,10 +147,10 @@ def run_cuda(lib, trace: traces.Trace, num_blocks: int, *, block_size: int = 512
     try:
         if store_seed is not None:
             init = traces.pattern_bytes(store_seed, 0, num_blocks * block_size)
-            for rep in ((0, 1) if mirror else (0,)):
+            for rep in range(replicas if mirror else 1):
                 lib.bdev_write_raw(bname, 0, init, replica=rep)
         if mirror:
-            assert lib.get_bdevs(bname)[0]["replicas"] == 2
+            assert lib.get_bdevs(bname)[0]["replicas"] == replicas
         if histogram:
             lib.enable_bdev_histogram(bname, True)
         with environ(**(kernel_env(kernel) if kernel is not None else {})), \
@@ -177,9 +178,9 @@ def run_cuda(lib, trace: traces.Trace, num_blocks: int, *, block_size: int = 512
                 shared = lun.shared_launches
                 assert shared == (kernel in SHARED_KERNELS), f"kernel={kernel}: the launch was {'' if shared else 'not '}shared"
         store = lib.bdev_read_raw(bname, 0, num_blocks * block_size)
-        if mirror:
-            assert (lib.bdev_read_raw(bname, 0, num_blocks * block_size, replica=1) == store).all(), \
-                f"kernel={kernel}: replica 1 differs from replica 0"
+        for rep in range(1, replicas if mirror else 1):
+            bad = np.nonzero(lib.bdev_read_raw(bname, 0, num_blocks * block_size, replica=rep) != store)[0]
+            assert not len(bad), f"kernel={kernel}: replica {rep} of {replicas} differs from replica 0 at {len(bad)} bytes, first {bad[:8]}"
         return cpls, arena, store, stats
     finally:
         lib.remove_vhost_scsi_target(cname, target)
