@@ -199,6 +199,19 @@ int oimgpu_bdev_create_mirror(const char *name, uint64_t num_blocks, uint32_t bl
 int oimgpu_bdev_export_store(const char *name, int replica, void *handle_out);
 int oimgpu_bdev_create_mirror_remote(const char *name, uint64_t num_blocks, uint32_t block_size, int device,
 				     const void *peer_handles, int npeers, char *name_out, size_t name_cap);
+/* The two constructors above with the bdev's uuid (NULL: random, as for the functions without it; otherwise as
+ * construct_malloc_bdev checks it), so that a restored configuration keeps the volume's identity.  In
+ * oimgpu_bdev_create_mirror_uuid, devices == NULL places the replicas by rule: replica 0 on the GPU
+ * construct_malloc_bdev would pick (least loaded), replica r on the r-th next initialised GPU, wrapping around.
+ * -ENOTSUP: a replica's GPU is not peer-reachable from replica 0's.  The remote form returns -EIO when a handle
+ * cannot be opened. */
+int oimgpu_bdev_create_mirror_uuid(const char *name, const char *uuid, uint64_t num_blocks, uint32_t block_size,
+				   const int *devices, int nreplicas, char *name_out, size_t name_cap);
+int oimgpu_bdev_create_mirror_remote_uuid(const char *name, const char *uuid, uint64_t num_blocks, uint32_t block_size,
+					  int device, const void *peer_handles, int npeers, char *name_out, size_t name_cap);
+/* where replica r of a bdev lives: its CUDA ordinal (an imported replica: the GPU it is reached from) and whether it is
+ * another process's store; -ENODEV unknown bdev, -EINVAL no such replica */
+int oimgpu_bdev_replica_info(const char *name, int replica, int *device, int *imported);
 /* Position-keyed 128-bit digest of [offset, offset+nbytes) of one replica's store (offset and nbytes multiples of
  * 8): out[0] = sum of w_i * (2i+1), out[1] = sum of mix64(w_i ^ i) over the 64-bit words w_i, i counted from the
  * start of the range, all mod 2^64 (mix64 = the splitmix64 finaliser).  Test/bench infrastructure for the

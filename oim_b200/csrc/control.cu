@@ -282,21 +282,34 @@ extern "C" int oimgpu_bdev_create_rbd(const char *name, const char *pool_name, c
 extern "C" int oimgpu_bdev_create_mirror(const char *name, uint64_t num_blocks, uint32_t block_size,
 					 const int *devices, int nreplicas, char *name_out, size_t name_cap)
 {
+	if (!devices) return -EINVAL;	/* placement by rule is the uuid entry point's */
+	return oimgpu_bdev_create_mirror_uuid(name, nullptr, num_blocks, block_size, devices, nreplicas, name_out, name_cap);
+}
+
+extern "C" int oimgpu_bdev_create_mirror_uuid(const char *name, const char *uuid, uint64_t num_blocks, uint32_t block_size,
+					      const int *devices, int nreplicas, char *name_out, size_t name_cap)
+{
 	std::lock_guard<std::mutex> lk(g.mu);
 	if (!g.inited) return -ENODEV;
-	if (!devices || nreplicas < 1 || nreplicas > kMaxReplicas) return -EINVAL;
-	std::vector<int> devs(devices, devices + nreplicas);
+	if (nreplicas < 1 || nreplicas > kMaxReplicas) return -EINVAL;
+	std::vector<int> devs;
+	if (devices) {
+		devs.assign(devices, devices + nreplicas);
+	} else {
+		/* replica 0 where construct_malloc_bdev would put it, replica r on the r-th next initialised GPU */
+		const int first = find_device_slot(pick_device(-1));
+		for (int r = 0; r < nreplicas; r++) devs.push_back(g.devices[(first + r) % g.devices.size()].ordinal);
+	}
 	for (int d : devs) {
 		if (find_device_slot(d) < 0) return -EINVAL;
 	}
 	for (int r = 1; r < nreplicas; r++) {
 		int can = 0;
-		cudaDeviceCanAccessPeer(&can, devs[0], devs[r]);
-		if (!can && devs[0] != devs[r]) return -ENOTSUP;
+		if (devs[0] != devs[r] && (cudaDeviceCanAccessPeer(&can, devs[0], devs[r]) != cudaSuccess || !can)) return -ENOTSUP;
 	}
 	std::string auto_name;
 	if (!(name && name[0])) auto_name = "Mirror" + std::to_string(g.malloc_disk_count);
-	int rc = create_bdev_locked(name, nullptr, num_blocks, block_size, devs, "Malloc disk", auto_name, name_out, name_cap);
+	int rc = create_bdev_locked(name, uuid, num_blocks, block_size, devs, "Malloc disk", auto_name, name_out, name_cap);
 	if (rc == 0 && !(name && name[0])) g.malloc_disk_count++;
 	return rc;
 }
@@ -320,6 +333,14 @@ extern "C" int oimgpu_bdev_export_store(const char *name, int replica, void *han
 extern "C" int oimgpu_bdev_create_mirror_remote(const char *name, uint64_t num_blocks, uint32_t block_size, int device,
 						 const void *peer_handles, int npeers, char *name_out, size_t name_cap)
 {
+	return oimgpu_bdev_create_mirror_remote_uuid(name, nullptr, num_blocks, block_size, device, peer_handles, npeers,
+						     name_out, name_cap);
+}
+
+extern "C" int oimgpu_bdev_create_mirror_remote_uuid(const char *name, const char *uuid, uint64_t num_blocks,
+						     uint32_t block_size, int device, const void *peer_handles, int npeers,
+						     char *name_out, size_t name_cap)
+{
 	std::lock_guard<std::mutex> lk(g.mu);
 	if (!g.inited || g.control_only) return -ENODEV;
 	if (!peer_handles || npeers < 1 || npeers >= kMaxReplicas) return -EINVAL;
@@ -328,7 +349,7 @@ extern "C" int oimgpu_bdev_create_mirror_remote(const char *name, uint64_t num_b
 	std::string auto_name;
 	if (!(name && name[0])) auto_name = "Mirror" + std::to_string(g.malloc_disk_count);
 	char nm[64];
-	int rc = create_bdev_locked(name, nullptr, num_blocks, block_size, {d}, "Malloc disk", auto_name, nm, sizeof(nm));
+	int rc = create_bdev_locked(name, uuid, num_blocks, block_size, {d}, "Malloc disk", auto_name, nm, sizeof(nm));
 	if (rc) return rc;
 	if (!(name && name[0])) g.malloc_disk_count++;
 	Bdev &b = *g.bdevs[nm];
@@ -349,8 +370,21 @@ extern "C" int oimgpu_bdev_create_mirror_remote(const char *name, uint64_t num_b
 		b.devices.push_back(d);
 		b.stores.push_back((uint8_t *)p);
 		b.imported.push_back(1);
+		b.ipc_handles.emplace_back((const char *)&h, sizeof(h));
 	}
 	copy_str(name_out, name_cap, nm);
+	return 0;
+}
+
+extern "C" int oimgpu_bdev_replica_info(const char *name, int replica, int *device, int *imported)
+{
+	std::lock_guard<std::mutex> lk(g.mu);
+	if (!g.inited) return -ENODEV;
+	Bdev *b = find_bdev_locked(name);
+	if (!b) return -ENODEV;
+	if (replica < 0 || replica >= (int)b->stores.size()) return -EINVAL;
+	if (device) *device = b->devices[replica];
+	if (imported) *imported = b->imported[replica];
 	return 0;
 }
 
@@ -783,6 +817,22 @@ static std::string json_escape(const std::string &in)
 	return o + "\"";
 }
 
+static std::string base64(const std::string &in)
+{
+	static const char tbl[] = "ABCDEFGHIJKLMNOPQRSTUVWXYZabcdefghijklmnopqrstuvwxyz0123456789+/";
+	const uint8_t *p = (const uint8_t *)in.data();
+	const size_t n = in.size();
+	std::string o;
+	for (size_t i = 0; i < n; i += 3) {
+		const uint32_t v = (uint32_t)p[i] << 16 | (i + 1 < n ? (uint32_t)p[i + 1] << 8 : 0) | (i + 2 < n ? p[i + 2] : 0);
+		o += tbl[v >> 18];
+		o += tbl[(v >> 12) & 63];
+		o += i + 1 < n ? tbl[(v >> 6) & 63] : '=';
+		o += i + 2 < n ? tbl[v & 63] : '=';
+	}
+	return o;
+}
+
 /* get_subsystem_config (S/lib/event/rpc/subsystem_rpc.c:80-129): the RPC calls that would rebuild the subsystem's
  * present state, as a JSON array of {"method", "params"} - spdk_bdev_subsystem_config_json (S/lib/bdev/bdev.c:676-708)
  * with bdev_malloc_write_json_config (bdev_malloc.c:350-368) / bdev_rbd_write_config_json (bdev_rbd.c:635-666), and
@@ -802,6 +852,18 @@ extern "C" long oimgpu_config_json(const char *subsystem, char *buf, size_t cap)
 				       json_escape(b.pool_name) + ",\"rbd_name\":" + json_escape(b.rbd_name) + ",\"block_size\":" + std::to_string(b.block_size);
 				if (!b.user_id.empty()) out += ",\"user_id\":" + json_escape(b.user_id);
 				out += "}}";
+			} else if (b.stores.size() > 1) {
+				/* a mirror: in-process replicas are placed again by the rule, imported ones opened again from their
+				 * handles (which stay valid while the exporting process keeps its bdev) */
+				out += ",{\"method\":\"construct_mirror_bdev\",\"params\":{\"name\":" + json_escape(b.name) + ",\"num_blocks\":" +
+				       std::to_string(b.num_blocks) + ",\"block_size\":" + std::to_string(b.block_size) + ",\"uuid\":" + json_escape(b.uuid);
+				if (b.ipc_handles.empty()) {
+					out += ",\"replicas\":" + std::to_string(b.stores.size()) + "}}";
+				} else {
+					out += ",\"remote_replicas\":[";
+					for (size_t k = 0; k < b.ipc_handles.size(); k++) out += (k ? ",\"" : "\"") + base64(b.ipc_handles[k]) + "\"";
+					out += "]}}";
+				}
 			} else {
 				out += ",{\"method\":\"construct_malloc_bdev\",\"params\":{\"name\":" + json_escape(b.name) + ",\"num_blocks\":" +
 				       std::to_string(b.num_blocks) + ",\"block_size\":" + std::to_string(b.block_size) + ",\"uuid\":" + json_escape(b.uuid) + "}}";

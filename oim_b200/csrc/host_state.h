@@ -51,6 +51,7 @@ struct Bdev {
 	std::vector<int> devices;	/* replica r lives on devices[r] (an imported replica: the device it is reached from) */
 	std::vector<uint8_t *> stores;
 	std::vector<char> imported;	/* replica r is another process's store, opened from a CUDA IPC handle */
+	std::vector<std::string> ipc_handles;	/* the handles the imported replicas were opened from, in replica order (config dump) */
 	unsigned long long *hist = nullptr;	/* enable_bdev_histogram: kHistBuckets counters on devices[0] */
 	unsigned long long retired[12] = {};	/* counters of sessions that are gone (same layout as LunCtx::stats) */
 };

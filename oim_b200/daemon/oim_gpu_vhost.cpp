@@ -8,7 +8,8 @@
  *   bdev methods         S/lib/bdev/rpc/bdev_rpc.c:216-433, S/lib/bdev/malloc/bdev_malloc_rpc.c:63-106,
  *                        S/lib/bdev/rbd/bdev_rbd_rpc.c:102-148
  *   vhost methods        S/lib/vhost/vhost_rpc.c:65-478
- * and is pinned against the reference's own server running in-process (tests/test_rpc_daemon.py).
+ * and is pinned against the reference's own server running in-process (tests/test_rpc_daemon.py).  Two methods are the
+ * project's own, for mirrored bdevs: construct_mirror_bdev and export_bdev_store (INTEGRATION.md 3c).
  *
  * CLI as S/app/vhost/vhost.c:43-48 + S/lib/event/app.c:826-960:
  *   -S <dir> vhost socket directory   -r <path> RPC socket (default /var/tmp/spdk.sock)
@@ -285,8 +286,60 @@ static std::string bdev_json(const oimgpu_bdev_info &b)
 	s += ",\"assigned_rate_limits\":{\"rw_ios_per_sec\":0,\"rw_mbytes_per_sec\":0,\"r_mbytes_per_sec\":0,\"w_mbytes_per_sec\":0}";
 	s += std::string(",\"claimed\":") + (b.claimed ? "true" : "false");
 	s += ",\"supported_io_types\":{\"read\":true,\"write\":true,\"unmap\":true,\"write_zeroes\":true,\"flush\":true,"
-	     "\"reset\":true,\"nvme_admin\":false,\"nvme_io\":false},\"driver_specific\":{}}";
-	return s;
+	     "\"reset\":true,\"nvme_admin\":false,\"nvme_io\":false},\"driver_specific\":{";
+	if (b.replicas > 1) {
+		/* a mirror (a project bdev: the reference has none) says where its replicas are */
+		s += "\"mirror\":{\"replicas\":[";
+		for (uint32_t r = 0; r < b.replicas; r++) {
+			int dev = 0, imported = 0;
+			oimgpu_bdev_replica_info(b.name, (int)r, &dev, &imported);
+			s += std::string(r ? "," : "") + "{\"gpu\":" + std::to_string(dev) + ",\"imported\":" + (imported ? "true" : "false") + "}";
+		}
+		s += "]}";
+	}
+	return s + "}}";
+}
+
+static std::string base64_encode(const uint8_t *p, size_t n)
+{
+	static const char tbl[] = "ABCDEFGHIJKLMNOPQRSTUVWXYZabcdefghijklmnopqrstuvwxyz0123456789+/";
+	std::string o;
+	o.reserve((n + 2) / 3 * 4);
+	for (size_t i = 0; i < n; i += 3) {
+		const uint32_t v = (uint32_t)p[i] << 16 | (i + 1 < n ? (uint32_t)p[i + 1] << 8 : 0) | (i + 2 < n ? p[i + 2] : 0);
+		o += tbl[v >> 18]; o += tbl[(v >> 12) & 63];
+		o += i + 1 < n ? tbl[(v >> 6) & 63] : '=';
+		o += i + 2 < n ? tbl[v & 63] : '=';
+	}
+	return o;
+}
+
+/* strict RFC 4648 base64 (padded, no whitespace); false on anything else */
+static bool base64_decode(const std::string &s, std::string *out)
+{
+	if (s.size() % 4) return false;
+	out->clear();
+	for (size_t i = 0; i < s.size(); i += 4) {
+		uint32_t v = 0;
+		int pad = 0;
+		for (int k = 0; k < 4; k++) {
+			const char c = s[i + k];
+			int d;
+			if (c >= 'A' && c <= 'Z') d = c - 'A';
+			else if (c >= 'a' && c <= 'z') d = c - 'a' + 26;
+			else if (c >= '0' && c <= '9') d = c - '0' + 52;
+			else if (c == '+') d = 62;
+			else if (c == '/') d = 63;
+			else if (c == '=' && i + 4 == s.size() && k >= 2) { d = 0; pad++; }
+			else return false;
+			if (pad && c != '=') return false;	/* nothing may follow padding */
+			v = v << 6 | (uint32_t)d;
+		}
+		*out += (char)(v >> 16);
+		if (pad < 2) *out += (char)(v >> 8 & 0xFF);
+		if (pad < 1) *out += (char)(v & 0xFF);
+	}
+	return true;
 }
 
 static std::string ctrlr_json(const oimgpu_ctrlr_info &c)
@@ -433,17 +486,7 @@ static Reply dispatch(const std::string &method, const Json *params, const Json 
 		int rc = oimgpu_bdev_histogram_get(a->raw.c_str(), buckets.data());
 		if (rc == -ENODEV) return error(id, E_INVALID_PARAMS, strerr(ENODEV));
 		if (rc < 0) return error(id, E_INTERNAL, strerr(rc));
-		static const char tbl[] = "ABCDEFGHIJKLMNOPQRSTUVWXYZabcdefghijklmnopqrstuvwxyz0123456789+/";
-		const uint8_t *p = (const uint8_t *)buckets.data();
-		const size_t n = buckets.size() * sizeof(uint64_t);
-		std::string b64;
-		b64.reserve((n + 2) / 3 * 4);
-		for (size_t i = 0; i < n; i += 3) {
-			const uint32_t v = (uint32_t)p[i] << 16 | (i + 1 < n ? (uint32_t)p[i + 1] << 8 : 0) | (i + 2 < n ? p[i + 2] : 0);
-			b64 += tbl[v >> 18]; b64 += tbl[(v >> 12) & 63];
-			b64 += i + 1 < n ? tbl[(v >> 6) & 63] : '=';
-			b64 += i + 2 < n ? tbl[v & 63] : '=';
-		}
+		const std::string b64 = base64_encode((const uint8_t *)buckets.data(), buckets.size() * sizeof(uint64_t));
 		return result(id, "{\"histogram\":\"" + b64 + "\",\"bucket_shift\":7,\"tsc_rate\":1000000000}");
 	}
 	if (method == "construct_malloc_bdev") {
@@ -468,6 +511,45 @@ static Reply dispatch(const std::string &method, const Json *params, const Json 
 						(uint32_t)bs, g_rbd_default_size, -1, name, sizeof(name));
 		if (rc != 0) return bad;
 		return result(id, jstr(name));
+	}
+	if (method == "construct_mirror_bdev") {
+		/* project method (the reference has no mirror, SURVEY.md 8(c)), shaped and answered like construct_malloc_bdev:
+		 * `replicas` in-process replicas placed by the library's rule, or replica 0 here and `remote_replicas` the
+		 * stores of other processes (base64 CUDA IPC handles, as export_bdev_store gives them) */
+		uint64_t nb = 0, bs = 0, nrep = 0;
+		if (!decode(params, {{"name", Json::Str, true, &a}, {"uuid", Json::Str, true, &b}, {"num_blocks", Json::Num, false, &c},
+				     {"block_size", Json::Num, false, &d}, {"replicas", Json::Num, true, &e}, {"remote_replicas", Json::Arr, true, &f}}))
+			return bad;
+		if (!to_u64(c, &nb) || !to_u64(d, &bs) || bs > UINT32_MAX || !e == !f) return bad;
+		const char *nm = a ? a->raw.c_str() : nullptr, *uuid = b ? b->raw.c_str() : nullptr;
+		char name[64];
+		int rc;
+		if (e) {
+			if (!to_u64(e, &nrep) || nrep < 2 || nrep > 4) return bad;
+			rc = oimgpu_bdev_create_mirror_uuid(nm, uuid, nb, (uint32_t)bs, nullptr, (int)nrep, name, sizeof(name));
+		} else {
+			if (f->arr.empty() || f->arr.size() > 3) return bad;
+			std::string handles, h;
+			for (auto &x : f->arr) {
+				if (x.type != Json::Str || !base64_decode(x.raw, &h) || h.size() != OIMGPU_IPC_HANDLE_BYTES) return bad;
+				handles += h;
+			}
+			rc = oimgpu_bdev_create_mirror_remote_uuid(nm, uuid, nb, (uint32_t)bs, -1, handles.data(), (int)f->arr.size(),
+								   name, sizeof(name));
+		}
+		if (rc != 0) return bad;
+		return result(id, jstr(name));
+	}
+	if (method == "export_bdev_store") {
+		/* the CUDA IPC handle of one replica's store, for another process's construct_mirror_bdev {remote_replicas}.
+		 * The bdev must outlive every mirror built on the handle: delete the importing mirror first. */
+		int32_t rep = 0;
+		if (!decode(params, {{"name", Json::Str, false, &a}, {"replica", Json::Num, true, &b}}) || (b && !to_i32(b, &rep)))
+			return error(id, E_INVALID_PARAMS, strerr(EINVAL));
+		uint8_t h[OIMGPU_IPC_HANDLE_BYTES];
+		int rc = oimgpu_bdev_export_store(a->raw.c_str(), rep, h);
+		if (rc < 0) return error(id, E_INVALID_PARAMS, strerr(rc));
+		return result(id, "\"" + base64_encode(h, sizeof(h)) + "\"");
 	}
 	if (method == "delete_bdev") {
 		if (!decode(params, {{"name", Json::Str, false, &a}})) return bad;

@@ -64,6 +64,9 @@ SYMBOLS = [
     ("oimgpu_bdev_create_mirror", _I, [C.c_char_p, _U64, _U32, C.POINTER(C.c_int), _I, C.c_char_p, C.c_size_t]),
     ("oimgpu_bdev_export_store", _I, [C.c_char_p, _I, _VP]),
     ("oimgpu_bdev_create_mirror_remote", _I, [C.c_char_p, _U64, _U32, _I, _VP, _I, C.c_char_p, C.c_size_t]),
+    ("oimgpu_bdev_create_mirror_uuid", _I, [C.c_char_p, C.c_char_p, _U64, _U32, C.POINTER(C.c_int), _I, C.c_char_p, C.c_size_t]),
+    ("oimgpu_bdev_create_mirror_remote_uuid", _I, [C.c_char_p, C.c_char_p, _U64, _U32, _I, _VP, _I, C.c_char_p, C.c_size_t]),
+    ("oimgpu_bdev_replica_info", _I, [C.c_char_p, _I, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     ("oimgpu_bdev_digest", _I, [C.c_char_p, _I, _U64, _U64, C.POINTER(C.c_uint64)]),
     ("oimgpu_digest_device", _I, [_I, _VP, _U64, C.POINTER(C.c_uint64)]),
     ("oimgpu_bdev_delete", _I, [C.c_char_p]),
