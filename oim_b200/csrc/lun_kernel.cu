@@ -1079,6 +1079,18 @@ static_assert(kSigBits == 1 << OIM_SIG_LOG2, "sig_index produces OIM_SIG_LOG2 bi
 
 /* ---- the kernel ----------------------------------------------------------------------------- */
 
+/* one lane: the ring cursors back into VqState - a virtqueue's avail and used index (16 significant bits), a slot
+ * ring's consumed position */
+__device__ __forceinline__ void store_cursors(VqState *vs, bool vring, uint32_t last_avail, uint32_t last_used)
+{
+	if (vring) {
+		vs->last_avail = last_avail & 0xffff;
+		vs->last_used = last_used & 0xffff;
+	} else {
+		vs->last_avail = last_avail;
+	}
+}
+
 /* parser side: publish the completions of the fill that occupied `st` (all movers are done with it) */
 /* pub_q / pub_end (shared kernels): the queue and end position this CTA published last - a fill that starts right
  * there has nothing of anybody else's to wait for */
@@ -1150,8 +1162,7 @@ __device__ __forceinline__ void reap_stage(Stage &st, int lane, QShare **pub_q =
 	if (st.share && lane == 0) {
 		if (!st.persistent && st.share_pos + n == st.share_final) {
 			/* last fill of this launch on the queue: everything before it is published - write the cursors back */
-			st.vq_state->last_avail = (st.share->base_avail + st.share_final) & 0xffff;
-			st.vq_state->last_used = (st.used_base + n) & 0xffff;
+			store_cursors(st.vq_state, true, st.share->base_avail + st.share_final, st.used_base + n);
 		}
 		st_release32(&st.share->done, st.share_pos + n);
 		if (pub_q) { *pub_q = st.share; *pub_end = st.share_pos + n; }
@@ -1173,28 +1184,53 @@ static __device__ __forceinline__ void mirror_unit(const LunCtx &L, uint8_t *dst
 	}
 }
 
+/* ---- queue positions ----------------------------------------------------------------------------------- */
+
+/* a queue's producer index: the host's tail doorbell (slot ring), the guest's avail->idx (virtqueue), or the
+ * dispatcher's mirror of either (hinted) */
+__device__ __forceinline__ uint32_t producer_index(const QueueDesc &q, bool hinted)
+{
+	if (hinted) return ld_vol32(&q.vq_state->hint);
+	return q.mode == QMODE_VRING ? (uint32_t)ld_vol16(q.vq_avail + 2) : ld_vol32(q.doorbell);
+}
+
+/* new entries on a virtqueue from ring position `from` up to avail index `idx` (16-bit arithmetic); 0 when there are
+ * more than the ring holds: "the queue is unrecoverably broken" */
+__device__ __forceinline__ uint32_t vq_new_entries(uint32_t idx, uint32_t from, uint32_t vq_size)
+{
+	const uint32_t k = (uint16_t)(idx - from);
+	return k > vq_size ? 0 : k;
+}
+
+/* one lane: the avail entry at ring position pos, i.e. the head of a request's chain.  Volatile, as every avail entry
+ * read: a resident CTA has this line in its L1 from the batch before, when the guest had not written it yet */
+__device__ __forceinline__ uint32_t vq_avail_entry(const QueueDesc &q, uint32_t pos)
+{
+	return reinterpret_cast<const volatile uint16_t *>(q.vq_avail + 4)[pos & (q.vq_size - 1)];
+}
+
+/* a lane whose request moves nothing: no request in this pass, or an invalid one */
+__device__ __forceinline__ void lane_reset(LaneState &s)
+{
+	s.op = OP_NONE; s.nseg = 0; s.units = 0; s.hazard = 0; s.valid = 0; s.store_lo = s.store_hi = 0;
+}
+
 /* ---- shared queues: who takes which pass --------------------------------------------------------------- */
 
 /* lane 0: take the next pass (<= 32 requests) of a shared queue.  Returns its length (0: nothing unclaimed right
  * now) and its position in *pos.  q.head = ring position of position 0; q.count = the launch's limit. */
-__device__ __forceinline__ uint32_t claim_pass(const QueueDesc &q, QShare &qs, bool persistent, bool hinted, uint32_t *pos,
+__device__ __forceinline__ uint32_t claim_pass(const QueueDesc &q, QShare *qs, bool persistent, bool hinted, uint32_t *pos,
 					       uint32_t want = kPass)
 {
 	for (;;) {
-		const uint32_t c = ld_vol32(&qs.claim);
+		const uint32_t c = ld_vol32(&qs->claim);
 		uint32_t avail;
-		if (!persistent) {
-			avail = q.count - c;
-		} else if (q.mode == QMODE_VRING) {
-			const uint16_t av = hinted ? (uint16_t)ld_vol32(&q.vq_state->hint) : ld_vol16(q.vq_avail + 2);
-			avail = (uint16_t)(av - (uint16_t)(q.head + c));
-			if (avail > q.vq_size) avail = 0;	/* "the queue is unrecoverably broken" */
-		} else {
-			avail = (hinted ? ld_vol32(&q.vq_state->hint) : ld_vol32(q.doorbell)) - (q.head + c);
-		}
+		if (!persistent) avail = q.count - c;
+		else if (q.mode == QMODE_VRING) avail = vq_new_entries(producer_index(q, hinted), q.head + c, q.vq_size);
+		else avail = producer_index(q, hinted) - (q.head + c);
 		if (avail == 0) return 0;
 		const uint32_t n = avail < want ? avail : want;
-		if (atomicCAS(&qs.claim, c, c + n) == c) {
+		if (atomicCAS(&qs->claim, c, c + n) == c) {
 			*pos = c;
 			return n;
 		}
@@ -1219,12 +1255,8 @@ __device__ __forceinline__ bool shared_queue_has_work(const QueueDesc &q, QShare
 		return c < q.count;
 	}
 	const uint32_t ring = ld_vol32(&qs.base_avail) + c;
-	if (q.mode == QMODE_VRING) {
-		const uint16_t av = hinted ? (uint16_t)ld_vol32(&q.vq_state->hint) : ld_vol16(q.vq_avail + 2);
-		const uint16_t k = (uint16_t)(av - (uint16_t)ring);
-		return k != 0 && k <= q.vq_size;
-	}
-	return (hinted ? ld_vol32(&q.vq_state->hint) : ld_vol32(q.doorbell)) != ring;
+	if (q.mode == QMODE_VRING) return vq_new_entries(producer_index(q, hinted), ring, q.vq_size) != 0;
+	return producer_index(q, hinted) != ring;
 }
 
 /* warp-wide: first queue with unclaimed work in cyclic order from `from` (0xffffffff: none), 32 queues per step */
@@ -1675,10 +1707,6 @@ __device__ __forceinline__ void lun_queue_body(LunCtx *lun, KickHeader *hdr, con
 		LaneState &s = sh.lane[lane];
 		uint32_t fills = 0;			/* stage fills so far */
 		uint32_t reaped = 0;			/* fills whose completions are published */
-		/* store ranges of the previous kStages-1 passes, per lane, for cross-pass hazards: movers are not
-		 * in lock-step, one may already work on pass p+2 while another is still in pass p (the stage ring
-		 * only stops the parser from refilling pass p's stage) */
-		constexpr int kHist = kStages - 1;
 		uint32_t pass_no = 0;			/* passes parsed by this CTA: index into the hazard history ring */
 		if (lane < kStages) { sh.hist[lane].writers = 0; sh.hist[lane].touching = 0; }
 		__syncwarp();
@@ -1805,8 +1833,7 @@ __device__ __forceinline__ void lun_queue_body(LunCtx *lun, KickHeader *hdr, con
 							 * (spdk_vhost_vq_avail_ring_get, vhost.c:178-211); the others wait for its word */
 							if (atomicCAS(&qs->latched, 0u, 2u) == 0u) {
 								const uint32_t la = q.vq_state->last_avail, lu = q.vq_state->last_used;
-								uint32_t c = (uint16_t)(ld_vol16(q.vq_avail + 2) - (uint16_t)la);
-								if (c > q.vq_size) c = 0;	/* "the queue is unrecoverably broken" */
+								const uint32_t c = vq_new_entries(producer_index(q, false), la, q.vq_size);
 								qs->base_avail = la; qs->base_used = lu; qs->count = c;
 								st_release32(&qs->latched, 1u);
 							} else {
@@ -1831,7 +1858,7 @@ __device__ __forceinline__ void lun_queue_body(LunCtx *lun, KickHeader *hdr, con
 				uint32_t cnt = 0, consumed = 0;
 				if (lane == 0) {
 					consumed = q.vq_state->last_avail;
-					cnt = (hinted ? ld_vol32(&q.vq_state->hint) : ld_vol32(q.doorbell)) - consumed;
+					cnt = producer_index(q, hinted) - consumed;
 				}
 				q.count = __shfl_sync(0xffffffffu, cnt, 0);
 				q.head = __shfl_sync(0xffffffffu, consumed, 0);
@@ -1841,8 +1868,7 @@ __device__ __forceinline__ void lun_queue_body(LunCtx *lun, KickHeader *hdr, con
 				if (lane == 0) {
 					vq_last_avail = q.vq_state->last_avail;
 					vq_last_used = q.vq_state->last_used;
-					cnt = (uint16_t)((hinted ? (uint16_t)ld_vol32(&q.vq_state->hint) : ld_vol16(q.vq_avail + 2)) - (uint16_t)vq_last_avail);
-					if (cnt > q.vq_size) cnt = 0;	/* "the queue is unrecoverably broken" */
+					cnt = vq_new_entries(producer_index(q, hinted), vq_last_avail, q.vq_size);
 				}
 				q.count = __shfl_sync(0xffffffffu, cnt, 0);
 				vq_last_avail = __shfl_sync(0xffffffffu, vq_last_avail, 0);
@@ -1867,9 +1893,7 @@ __device__ __forceinline__ void lun_queue_body(LunCtx *lun, KickHeader *hdr, con
 			int4 vq_raw = make_int4(0, 0, 0, 0);	/* desc[head] of the coming pass, still in flight */
 			const bool vq_tbl_aligned = ((uintptr_t)q.vq_desc & 15) == 0;
 			if (!shared && q.count && q.mode == QMODE_VRING && (uint32_t)lane < min((uint32_t)kPass, q.count)) {
-				/* volatile, as every avail entry read: a resident CTA has this line in its L1 from the batch before,
-				 * when the guest had not written these entries yet */
-				vq_head_cur = reinterpret_cast<const volatile uint16_t *>(q.vq_avail + 4)[(q.head + lane) & (q.vq_size - 1)];
+				vq_head_cur = vq_avail_entry(q, q.head + lane);
 				if (vq_tbl_aligned && vq_head_cur < q.vq_size) vq_raw = ld_cg16(q.vq_desc + (size_t)vq_head_cur * 16);
 			}
 			uint32_t done = 0;	/* position of the current pass on the queue */
@@ -1888,7 +1912,7 @@ __device__ __forceinline__ void lun_queue_body(LunCtx *lun, KickHeader *hdr, con
 				} else {
 					if (next_n == 0) {
 						uint32_t pos = 0, got = 0;
-						if (lane == 0) got = claim_pass(q, *qs, persistent, hinted, &pos);
+						if (lane == 0) got = claim_pass(q, qs, persistent, hinted, &pos);
 						next_n = __shfl_sync(0xffffffffu, got, 0);
 						if (next_n == 0) break;
 						next_done = __shfl_sync(0xffffffffu, pos, 0);
@@ -1897,7 +1921,7 @@ __device__ __forceinline__ void lun_queue_body(LunCtx *lun, KickHeader *hdr, con
 						if (q.mode == QMODE_SLOTS) {
 							issue_fetch(q, q.head + next_done, next_n);
 						} else if ((uint32_t)lane < next_n) {
-							vq_head_cur = reinterpret_cast<const volatile uint16_t *>(q.vq_avail + 4)[(q.head + next_done + lane) & (q.vq_size - 1)];
+							vq_head_cur = vq_avail_entry(q, q.head + next_done + lane);
 							if (vq_tbl_aligned && vq_head_cur < q.vq_size) vq_raw = ld_cg16(q.vq_desc + (size_t)vq_head_cur * 16);
 						}
 					}
@@ -1920,7 +1944,7 @@ __device__ __forceinline__ void lun_queue_body(LunCtx *lun, KickHeader *hdr, con
 				bool chain_ok = true;
 				const bool vq_more = q.mode == QMODE_VRING && (uint32_t)lane < min((uint32_t)kPass, ahead);
 				if (vq_more)	/* next pass's avail entries: in flight while this pass is walked */
-					vq_head_nxt = reinterpret_cast<const volatile uint16_t *>(q.vq_avail + 4)[(slot0 + n + lane) & (q.vq_size - 1)];
+					vq_head_nxt = vq_avail_entry(q, slot0 + n + lane);
 				if (q.mode == QMODE_VRING && active) {
 					my_head = vq_head_cur;
 					VDesc d0 = {0, 0, 0, 0};
@@ -1942,12 +1966,12 @@ __device__ __forceinline__ void lun_queue_body(LunCtx *lun, KickHeader *hdr, con
 				if (active && chain_ok) parse_request(L, q, rq[lane], s);
 				else if (active) {
 					/* invalid_request(): used element of length 0, response untouched (vhost_scsi.c:347-358) */
-					s.op = OP_NONE; s.nseg = 0; s.units = 0; s.hazard = 0; s.valid = 0; s.store_lo = s.store_hi = 0;
+					lane_reset(s);
 					s.length = 0; s.data_transferred = 0; s.used_len = 0; s.resp_valid = 0; s.response = 0;
 					s.status = SC_GOOD; s.sk = 0; s.asc = 0;
 					rq[lane].tag = 0; rq[lane].iovcnt = 0;
 				}
-				else { s.nseg = 0; s.units = 0; s.hazard = 0; s.op = OP_NONE; s.valid = 0; s.store_lo = s.store_hi = 0; }
+				else lane_reset(s);
 				const uint32_t haz = active ? s.hazard : 0;
 				const uint64_t lo = s.store_lo, hi = s.store_hi;
 
@@ -2009,7 +2033,7 @@ __device__ __forceinline__ void lun_queue_body(LunCtx *lun, KickHeader *hdr, con
 							chunk_left -= next_n;
 						} else {
 							uint32_t pos = 0, got = 0;
-							if (lane == 0) got = claim_pass(q, *qs, persistent, hinted, &pos, streak >= 2 ? 4u * kPass : (uint32_t)kPass);
+							if (lane == 0) got = claim_pass(q, qs, persistent, hinted, &pos, streak >= 2 ? 4u * kPass : (uint32_t)kPass);
 							got = __shfl_sync(0xffffffffu, got, 0);
 							next_done = __shfl_sync(0xffffffffu, pos, 0);
 							streak = (got && next_done == done + n) ? streak + 1 : 0;
@@ -2019,7 +2043,7 @@ __device__ __forceinline__ void lun_queue_body(LunCtx *lun, KickHeader *hdr, con
 						if (next_n && q.mode == QMODE_SLOTS) {
 							issue_fetch(q, q.head + next_done, next_n);
 						} else if (next_n && (uint32_t)lane < next_n) {
-							vq_head_nxt = reinterpret_cast<const volatile uint16_t *>(q.vq_avail + 4)[(q.head + next_done + lane) & (q.vq_size - 1)];
+							vq_head_nxt = vq_avail_entry(q, q.head + next_done + lane);
 							if (vq_tbl_aligned && vq_head_nxt < q.vq_size) vq_raw = ld_cg16(q.vq_desc + (size_t)vq_head_nxt * 16);
 						}
 					}
@@ -2132,10 +2156,9 @@ __device__ __forceinline__ void lun_queue_body(LunCtx *lun, KickHeader *hdr, con
 				/* the parser owns both cursors: every consumed avail entry has its used element at vq_last_used + its
 				 * position, published or not.  A resident CTA that comes straight back to this ring while the movers
 				 * still hold the batch must place the next one behind it, not where publication has got to */
-				q.vq_state->last_avail = (vq_last_avail + q.count) & 0xffff;
-				q.vq_state->last_used = (vq_last_used + q.count) & 0xffff;
+				store_cursors(q.vq_state, true, vq_last_avail + q.count, vq_last_used + q.count);
 			}
-			if (!shared && persistent && q.mode == QMODE_SLOTS && lane == 0) q.vq_state->last_avail = q.head + q.count;
+			if (!shared && persistent && q.mode == QMODE_SLOTS && lane == 0) store_cursors(q.vq_state, false, q.head + q.count, 0);
 		}
 		/* tell the movers to stop, then publish the completions still in flight */
 		{
@@ -2157,14 +2180,10 @@ __device__ __forceinline__ void lun_queue_body(LunCtx *lun, KickHeader *hdr, con
 			if (__shfl_sync(0xffffffffu, last, 0)) {
 				__threadfence();
 				for (uint32_t k = lane; k < nqueues; k += 32) {
-					const QueueDesc &d = queues[k];
+					const bool vring = queues[k].mode == QMODE_VRING;
 					const uint32_t c = ld_vol32(&shares[k].claim);
-					if (d.mode == QMODE_VRING) {
-						d.vq_state->last_avail = (ld_vol32(&shares[k].base_avail) + c) & 0xffff;
-						d.vq_state->last_used = (ld_vol32(&shares[k].base_used) + c) & 0xffff;
-					} else {
-						d.vq_state->last_avail = ld_vol32(&shares[k].base_avail) + c;
-					}
+					const uint32_t la = ld_vol32(&shares[k].base_avail) + c;
+					store_cursors(queues[k].vq_state, vring, la, vring ? ld_vol32(&shares[k].base_used) + c : 0);
 				}
 				__threadfence();
 			}
