@@ -218,6 +218,23 @@ int oimgpu_bdev_replica_info(const char *name, int replica, int *device, int *im
  * size-independent parity properties (replica == replica == expected content) at sizes a host copy is too slow for. */
 int oimgpu_bdev_digest(const char *name, int replica, uint64_t offset, uint64_t nbytes, uint64_t out[2]);
 int oimgpu_digest_device(int device, const void *dev_ptr, uint64_t nbytes, uint64_t out[2]);
+/* check / repair of a mirrored bdev, as md RAID1's `check` and `repair` (mismatch_cnt): an exact block-by-block compare
+ * of every replica with replica 0, on replica 0's GPU. */
+struct oimgpu_mirror_check {
+	uint64_t blocks_checked, mismatched_blocks, repaired_blocks;
+	uint32_t nranges;	/* ranges written to `ranges` */
+	uint32_t truncated;	/* more ranges than max_ranges */
+};
+/* Compare every replica of a mirrored bdev with replica 0 over [offset_blocks, offset_blocks + num_blocks); with
+ * repair != 0, copy replica 0 over each block that differs.  ranges: max_ranges pairs {offset_blocks, num_blocks} of
+ * differing blocks in LBA order.  -ENODEV no such bdev / control-only, -ENOTSUP not a mirror, -EINVAL range outside
+ * the bdev or NULL out, -EBUSY an NBD export is serving it.
+ * Quiescence: every session that reaches the bdev (and every session on replica 0's GPU) is held for the call, its
+ * resident poller parked and restarted afterwards, and what it launched is waited for.  Writers in ANOTHER process - the
+ * exporter of an imported replica writing its own bdev - are not paused: quiesce them first, or the result describes
+ * a moment of the race and a repair may undo their writes. */
+int oimgpu_bdev_mirror_check(const char *name, uint64_t offset_blocks, uint64_t num_blocks, int repair,
+			     uint64_t *ranges, uint32_t max_ranges, struct oimgpu_mirror_check *out);
 int oimgpu_bdev_delete(const char *name);			/* -ENODEV if unknown; attached targets are hot-removed
 								 * (as spdk_bdev_unregister does); -EBUSY while a
 								 * data path (oimgpu_lun) is open on it */

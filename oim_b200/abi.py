@@ -68,6 +68,11 @@ bio_dtype = np.dtype([("offset_blocks", "<u8"), ("num_blocks", "<u8"), ("op", "<
 bio_cpl_dtype = np.dtype([("tag", "<u8"), ("status", "<i4"), ("pad", "<u4")])
 assert bio_dtype.itemsize == 40 and bio_cpl_dtype.itemsize == 16
 
+# check / repair of a mirrored bdev (oimgpu_bdev_mirror_check): struct oimgpu_mirror_check
+mirror_check_dtype = np.dtype([("blocks_checked", "<u8"), ("mismatched_blocks", "<u8"), ("repaired_blocks", "<u8"),
+                               ("nranges", "<u4"), ("truncated", "<u4")])
+assert mirror_check_dtype.itemsize == 32
+
 # completion fields the reference defines (everything but our bookkeeping extras)
 CPL_PARITY_FIELDS = ("tag", "sense_len", "resid", "status_qualifier", "status", "response",
                      "sense", "resp_valid", "used_len")

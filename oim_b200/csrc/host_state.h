@@ -1,5 +1,6 @@
 /*
- * host_state.h - what the host-side files of liboimgpu.so (control.cu, session.cu, nbd.cu, copy_chan.cu) share:
+ * host_state.h - what the host-side files of liboimgpu.so (control.cu, session.cu, nbd.cu, copy_chan.cu, bio_chan.cu,
+ * mirror_check.cu) share:
  * the registry, the session, and the helpers more than one of them calls.  Internal, not installed.
  */
 #pragma once
@@ -48,6 +49,7 @@ struct Bdev {
 	uint32_t block_size = 0;
 	int claimed = 0;	/* number of SCSI targets built on it */
 	int open_luns = 0;	/* oimgpu_lun handles */
+	int nbd_exports = 0;	/* oimgpu_nbd_serve calls serving it (also counted in open_luns) */
 	std::vector<int> devices;	/* replica r lives on devices[r] (an imported replica: the device it is reached from) */
 	std::vector<uint8_t *> stores;
 	std::vector<char> imported;	/* replica r is another process's store, opened from a CUDA IPC handle */
@@ -201,13 +203,16 @@ struct ParkedPollers {
 	/* device < 0: every GPU (pinned host memory is mapped into all of them) */
 	explicit ParkedPollers(int device, oimgpu_lun *except = nullptr)
 	{
-		for (oimgpu_lun *L : g.handles) {
-			if (L == except || (device >= 0 && L->device != device)) continue;
-			L->mu.lock();
-			const bool was = L->poller_active;
-			if (was) oimgpu_lun_stop_poller(L);
-			parked.push_back({L, was});
-		}
+		park([&](const oimgpu_lun *L) { return L != except && (device < 0 || L->device == device); });
+	}
+	/* every session on GPU `device`, and every session that reaches bdev `bdev` (its own device or a peer target) */
+	ParkedPollers(int device, const std::string &bdev)
+	{
+		park([&](const oimgpu_lun *L) {
+			if (L->device == device || L->bdev == bdev) return true;
+			for (const std::string &p : L->peer_bdev) if (p == bdev) return true;
+			return false;
+		});
 	}
 	~ParkedPollers()
 	{
@@ -221,5 +226,17 @@ struct ParkedPollers {
 
 	struct Session { oimgpu_lun *L; bool restart; };
 	std::vector<Session> parked;
+
+private:
+	template <class Want> void park(Want want)
+	{
+		for (oimgpu_lun *L : g.handles) {
+			if (!want(L)) continue;
+			L->mu.lock();
+			const bool was = L->poller_active;
+			if (was) oimgpu_lun_stop_poller(L);
+			parked.push_back({L, was});
+		}
+	}
 };
 

@@ -55,6 +55,7 @@ extern "C" int oimgpu_nbd_serve(const char *bdev_name, int sock_fd)
 		size = b.num_blocks * (uint64_t)b.block_size;
 		bs = b.block_size;
 		b.open_luns++;		/* pins the bdev like a session does */
+		b.nbd_exports++;	/* and refuses a mirror check: this loop cannot be paused */
 	}
 	int rc = 0;
 	cudaStream_t st = nullptr;
@@ -129,6 +130,7 @@ extern "C" int oimgpu_nbd_serve(const char *bdev_name, int sock_fd)
 		}
 		Bdev *b = find_bdev_locked(name.c_str());
 		if (b && b->open_luns > 0) b->open_luns--;
+		if (b && b->nbd_exports > 0) b->nbd_exports--;
 	}
 	if (st) cudaStreamDestroy(st);
 	return rc;

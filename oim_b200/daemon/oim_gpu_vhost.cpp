@@ -8,8 +8,8 @@
  *   bdev methods         S/lib/bdev/rpc/bdev_rpc.c:216-433, S/lib/bdev/malloc/bdev_malloc_rpc.c:63-106,
  *                        S/lib/bdev/rbd/bdev_rbd_rpc.c:102-148
  *   vhost methods        S/lib/vhost/vhost_rpc.c:65-478
- * and is pinned against the reference's own server running in-process (tests/test_rpc_daemon.py).  Two methods are the
- * project's own, for mirrored bdevs: construct_mirror_bdev and export_bdev_store (INTEGRATION.md 3c).
+ * and is pinned against the reference's own server running in-process (tests/test_rpc_daemon.py).  Three methods are the
+ * project's own, for mirrored bdevs: construct_mirror_bdev, export_bdev_store and check_mirror_bdev (INTEGRATION.md 3c).
  *
  * CLI as S/app/vhost/vhost.c:43-48 + S/lib/event/app.c:826-960:
  *   -S <dir> vhost socket directory   -r <path> RPC socket (default /var/tmp/spdk.sock)
@@ -550,6 +550,32 @@ static Reply dispatch(const std::string &method, const Json *params, const Json 
 		int rc = oimgpu_bdev_export_store(a->raw.c_str(), rep, h);
 		if (rc < 0) return error(id, E_INVALID_PARAMS, strerr(rc));
 		return result(id, "\"" + base64_encode(h, sizeof(h)) + "\"");
+	}
+	if (method == "check_mirror_bdev") {
+		/* compare every replica with replica 0 (and copy replica 0 over the blocks that differ, with repair): md RAID1's
+		 * check / repair.  At most kMaxRanges runs of differing blocks are listed; mismatched_blocks counts them all. */
+		constexpr uint32_t kMaxRanges = 64;
+		uint64_t off = 0, n = 0;
+		if (!decode(params, {{"name", Json::Str, false, &a}, {"offset_blocks", Json::Num, true, &b}, {"num_blocks", Json::Num, true, &c},
+				     {"repair", Json::Bool, true, &d}}) || (b && !to_u64(b, &off)) || (c && !to_u64(c, &n)))
+			return bad;
+		oimgpu_bdev_info info;
+		int rc = oimgpu_bdev_get(a->raw.c_str(), &info);
+		if (rc < 0) return error(id, E_INVALID_PARAMS, strerr(rc));
+		if (!c) n = off <= info.num_blocks ? info.num_blocks - off : 0;
+		uint64_t ranges[2 * kMaxRanges];
+		oimgpu_mirror_check res;
+		rc = oimgpu_bdev_mirror_check(a->raw.c_str(), off, n, d && d->b, ranges, kMaxRanges, &res);
+		if (rc < 0) return error(id, E_INVALID_PARAMS, strerr(rc));
+		std::string out = "{\"name\":" + jstr(info.name) + ",\"replicas\":" + std::to_string(info.replicas) +
+				  ",\"offset_blocks\":" + std::to_string(off) + ",\"num_blocks\":" + std::to_string(n) +
+				  ",\"mismatched_blocks\":" + std::to_string(res.mismatched_blocks) +
+				  ",\"repaired_blocks\":" + std::to_string(res.repaired_blocks) + ",\"mismatches\":[";
+		for (uint32_t k = 0; k < res.nranges; k++) {
+			out += std::string(k ? "," : "") + "{\"offset_blocks\":" + std::to_string(ranges[2 * k]) +
+			       ",\"num_blocks\":" + std::to_string(ranges[2 * k + 1]) + "}";
+		}
+		return result(id, out + "],\"truncated\":" + (res.truncated ? "true" : "false") + "}");
 	}
 	if (method == "delete_bdev") {
 		if (!decode(params, {{"name", Json::Str, false, &a}})) return bad;

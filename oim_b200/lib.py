@@ -69,6 +69,7 @@ SYMBOLS = [
     ("oimgpu_bdev_replica_info", _I, [C.c_char_p, _I, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     ("oimgpu_bdev_digest", _I, [C.c_char_p, _I, _U64, _U64, C.POINTER(C.c_uint64)]),
     ("oimgpu_digest_device", _I, [_I, _VP, _U64, C.POINTER(C.c_uint64)]),
+    ("oimgpu_bdev_mirror_check", _I, [C.c_char_p, _U64, _U64, _I, _VP, _U32, _VP]),
     ("oimgpu_bdev_delete", _I, [C.c_char_p]),
     ("oimgpu_bdev_get", _I, [C.c_char_p, C.POINTER(BdevInfo)]),
     ("oimgpu_bdev_list", _I, [C.POINTER(BdevInfo), _I]),
@@ -252,6 +253,24 @@ def digest_host(data: np.ndarray) -> tuple[int, int]:
         z = z ^ (z >> np.uint64(31))
         b = int(z.sum(dtype=np.uint64))
     return a, b
+
+
+def mirror_check(name: str, offset_blocks: int = 0, num_blocks: int | None = None, repair: bool = False,
+                 max_ranges: int = 64) -> dict:
+    """compare every replica of a mirrored bdev with replica 0 over [offset_blocks, offset_blocks + num_blocks) (default:
+    to the end); repair=True copies replica 0 over each block that differs (include/oimgpu.h oimgpu_bdev_mirror_check).
+    ranges: the first max_ranges runs of differing blocks, (offset_blocks, num_blocks) in LBA order."""
+    if num_blocks is None:
+        num_blocks = max(get_bdevs(name)[0]["num_blocks"] - offset_blocks, 0)
+    out = np.zeros(1, dtype=abi.mirror_check_dtype)
+    ranges = np.zeros(2 * max(max_ranges, 1), dtype=np.uint64)
+    _chk(load().oimgpu_bdev_mirror_check(_b(name), offset_blocks, num_blocks, int(repair), ranges.ctypes.data, max_ranges,
+                                         out.ctypes.data), "mirror_check")
+    o = out[0]
+    n = int(o["nranges"])
+    return {"blocks_checked": int(o["blocks_checked"]), "mismatched_blocks": int(o["mismatched_blocks"]),
+            "repaired_blocks": int(o["repaired_blocks"]),
+            "ranges": [(int(ranges[2 * i]), int(ranges[2 * i + 1])) for i in range(n)], "truncated": bool(o["truncated"])}
 
 
 def delete_bdev(name: str) -> None:
