@@ -212,6 +212,21 @@ int oimgpu_bdev_create_mirror_remote_uuid(const char *name, const char *uuid, ui
 /* where replica r of a bdev lives: its CUDA ordinal (an imported replica: the GPU it is reached from) and whether it is
  * another process's store; -ENODEV unknown bdev, -EINVAL no such replica */
 int oimgpu_bdev_replica_info(const char *name, int replica, int *device, int *imported);
+/* Move replica `replica` (1 .. nreplicas-1) of a mirror built with remote replicas to the store behind `handle`
+ * (OIMGPU_IPC_HANDLE_BYTES bytes, as oimgpu_bdev_export_store gives them), as mdadm --replace does: replica 0's bytes
+ * are copied into the new store on replica 0's GPU, every session of this process is pointed at it, and the old
+ * mapping is closed.  On return every session writes to the new store and none can reach the old one; the replica is
+ * still imported, reached from the same GPU, and the counters, histogram, uuid and targets of the bdev are unchanged.
+ * -EINVAL NULL argument, replica out of range, or a handle that is already one of the mirror's; -ENODEV no such bdev /
+ * control-only; -ENOTSUP not a mirror, a mirror with in-process replicas, or the new store's GPU not peer-reachable
+ * from replica 0's; -EIO the handle does not open (the mirror is unchanged and keeps serving on the old replica);
+ * -EBUSY an NBD export is serving the bdev.  On every failure the mirror is left as it was.
+ * Quiescence: as oimgpu_bdev_mirror_check, every session that reaches the bdev (and every session on replica 0's GPU)
+ * is held for the call - resident pollers parked and restarted, launched work waited for - so a guest sees one stall
+ * of the call's length.  Writers in ANOTHER process are not paused.  The new store must hold at least the bdev's
+ * num_blocks * block_size bytes, which nothing here can check.  The old exporter must keep its bdev until the call
+ * returns and may delete it afterwards: this is a planned move, not recovery from a dead peer. */
+int oimgpu_bdev_mirror_replace_remote(const char *name, int replica, const void *handle);
 /* Position-keyed 128-bit digest of [offset, offset+nbytes) of one replica's store (offset and nbytes multiples of
  * 8): out[0] = sum of w_i * (2i+1), out[1] = sum of mix64(w_i ^ i) over the 64-bit words w_i, i counted from the
  * start of the range, all mod 2^64 (mix64 = the splitmix64 finaliser).  Test/bench infrastructure for the

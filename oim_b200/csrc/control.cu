@@ -388,6 +388,74 @@ extern "C" int oimgpu_bdev_replica_info(const char *name, int replica, int *devi
 	return 0;
 }
 
+/* A planned move of an imported replica (mdadm --replace): the new store is filled from replica 0 and swapped in with
+ * every session that reaches the mirror held, so no request ever sees a replica that is missing or behind. */
+extern "C" int oimgpu_bdev_mirror_replace_remote(const char *name, int replica, const void *handle)
+{
+	if (!name || !handle) return -EINVAL;
+	std::lock_guard<std::mutex> lk(g.mu);
+	if (!g.inited || g.control_only) return -ENODEV;
+	Bdev *b = find_bdev_locked(name);
+	if (!b) return -ENODEV;
+	/* only a mirror built from handles: the configuration dump can then name the new store */
+	if (b->stores.size() < 2) return -ENOTSUP;
+	for (size_t r = 1; r < b->stores.size(); r++) {
+		if (!b->imported[r]) return -ENOTSUP;
+	}
+	if (replica < 1 || replica >= (int)b->stores.size()) return -EINVAL;
+	/* by its bytes, before it is opened: what the driver does with a handle this process holds open is not ours to rely on */
+	const std::string h((const char *)handle, OIMGPU_IPC_HANDLE_BYTES);
+	if (std::find(b->ipc_handles.begin(), b->ipc_handles.end(), h) != b->ipc_handles.end()) return -EINVAL;
+	if (b->nbd_exports) return -EBUSY;	/* an NBD export moves payload with no point at which it could be paused */
+
+	/* as oimgpu_bdev_mirror_check: every session that reaches the bdev, and every session on replica 0's GPU, held
+	 * and drained for the whole call */
+	const int dev0 = b->devices[0];
+	ParkedPollers held(dev0, b->name);
+	for (const auto &p : held.parked) {
+		CU_OK(cudaSetDevice(p.L->device));
+		CU_OK(cudaStreamSynchronize(p.L->stream));
+	}
+	CU_OK(cudaSetDevice(dev0));
+	cudaIpcMemHandle_t ih;
+	memcpy(&ih, handle, sizeof(ih));
+	void *p = nullptr;
+	cudaError_t e = cudaIpcOpenMemHandle(&p, ih, cudaIpcMemLazyEnablePeerAccess);
+	if (e != cudaSuccess) {
+		fprintf(stderr, "oimgpu: cudaIpcOpenMemHandle failed: %s\n", cudaGetErrorString(e));
+		(void)cudaGetLastError();
+		return e == cudaErrorPeerAccessUnsupported ? -ENOTSUP : -EIO;
+	}
+	uint8_t *fresh = (uint8_t *)p, *old = b->stores[replica];
+	auto drop = [&](int rc) {
+		cudaSetDevice(dev0);
+		cudaIpcCloseMemHandle(fresh);
+		(void)cudaGetLastError();
+		return rc;
+	};
+	cudaPointerAttributes at;
+	if (cudaPointerGetAttributes(&at, fresh) != cudaSuccess) return drop(-EIO);
+	if (!device_reachable(dev0, at.device)) return drop(-ENOTSUP);
+	const Device &dev = g.devices[find_device_slot(dev0)];
+	e = cudaSetDevice(dev0);
+	if (e == cudaSuccess) e = launch_copy(dev.util, dev.sm_count, fresh, b->stores[0], b->num_blocks * (uint64_t)b->block_size);
+	if (e == cudaSuccess) e = cudaStreamSynchronize(dev.util);
+	if (e != cudaSuccess) {
+		fprintf(stderr, "oimgpu: copy of %s replica 0 to its new replica %d failed: %s\n", b->name.c_str(), replica,
+			cudaGetErrorString(e));
+		return drop(-EIO);
+	}
+	int rc = publish_replica_locked(b->name, replica, fresh);
+	if (rc) {
+		publish_replica_locked(b->name, replica, old);
+		return drop(rc);
+	}
+	release_store(*b, (size_t)replica);
+	b->stores[replica] = fresh;
+	b->ipc_handles[replica - 1] = h;	/* replicas 1.. are all imported: handle k is replica k + 1's */
+	return 0;
+}
+
 /* Everything already launched on the sessions' streams comes first.  A resident poller cannot be waited for: with one
  * running, quiescing its I/O is the caller's business. */
 static int sync_session_streams_locked()

@@ -120,6 +120,7 @@ Ctrlr *find_ctrlr_locked(const char *ctrlr);	/* by ctrlr_key(ctrlr); nullptr: no
 bool read_ctx_stats(int device, const LunCtx *d_ctx, unsigned long long out[12]);
 void iostat_from_stats(const unsigned long long stats[12], oimgpu_iostat *out);
 void refresh_ctrlr_sessions_locked(const std::string &ctrlr);
+int publish_replica_locked(const std::string &bdev, int replica, uint8_t *store);	/* every LunCtx of the bdev */
 cudaError_t launch_copy(cudaStream_t st, int sm_count, void *dst, const void *src, uint64_t nbytes);
 cudaError_t launch_fill(cudaStream_t st, int sm_count, void *dst, uint8_t fill, uint64_t nbytes);
 void unpin_all_host_ranges();	/* oimgpu_mem_ensure's registrations */

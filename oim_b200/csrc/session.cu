@@ -148,6 +148,31 @@ void oimgpu::refresh_ctrlr_sessions_locked(const std::string &ctrlr)
 	}
 }
 
+/* Point store[replica] of every device-resident context of bdev `bdev` - a session's own and the peer-target contexts
+ * of controller-wide sessions - at `store`.  refresh_peers_locked rebuilds a context only when a target's bdev name
+ * changes, so a store that changes under the same name needs this.  Caller holds g.mu and has held and drained every
+ * session that reaches the bdev: no kernel reads a context while it changes.  The host copy of a session's own context
+ * changes too, since oimgpu_lun_set_removed and oimgpu_lun_set_mem_table upload it whole. */
+int oimgpu::publish_replica_locked(const std::string &bdev, int replica, uint8_t *store)
+{
+	const size_t at = offsetof(LunCtx, store) + sizeof(uint8_t *) * replica;
+	for (oimgpu_lun *L : g.handles) {
+		std::lock_guard<std::recursive_mutex> hl(L->mu);
+		CU_OK(cudaSetDevice(L->device));
+		if (L->bdev == bdev) {
+			L->h_ctx.store[replica] = store;
+			CU_OK(cudaMemcpyAsync((uint8_t *)L->d_ctx + at, &L->h_ctx.store[replica], sizeof(store), cudaMemcpyHostToDevice,
+					      L->copy_stream));
+		}
+		for (int t = 0; t < OIMGPU_CTRLR_MAX_DEVS; t++) {
+			if (L->peer_bdev[t] != bdev || !L->d_peer[t]) continue;
+			CU_OK(cudaMemcpyAsync((uint8_t *)L->d_peer[t] + at, &store, sizeof(store), cudaMemcpyHostToDevice, L->copy_stream));
+		}
+		CU_OK(cudaStreamSynchronize(L->copy_stream));	/* `store` is pageable */
+	}
+	return 0;
+}
+
 /* ---- data path ----------------------------------------------------------------------------------- */
 
 /* everything a session allocated, whether oimgpu_lun_open got through or not (every member starts null).

@@ -8,8 +8,9 @@
  *   bdev methods         S/lib/bdev/rpc/bdev_rpc.c:216-433, S/lib/bdev/malloc/bdev_malloc_rpc.c:63-106,
  *                        S/lib/bdev/rbd/bdev_rbd_rpc.c:102-148
  *   vhost methods        S/lib/vhost/vhost_rpc.c:65-478
- * and is pinned against the reference's own server running in-process (tests/test_rpc_daemon.py).  Three methods are the
- * project's own, for mirrored bdevs: construct_mirror_bdev, export_bdev_store and check_mirror_bdev (INTEGRATION.md 3c).
+ * and is pinned against the reference's own server running in-process (tests/test_rpc_daemon.py).  Four methods are the
+ * project's own, for mirrored bdevs: construct_mirror_bdev, export_bdev_store, check_mirror_bdev and
+ * replace_mirror_replica (INTEGRATION.md 3c).
  *
  * CLI as S/app/vhost/vhost.c:43-48 + S/lib/event/app.c:826-960:
  *   -S <dir> vhost socket directory   -r <path> RPC socket (default /var/tmp/spdk.sock)
@@ -576,6 +577,18 @@ static Reply dispatch(const std::string &method, const Json *params, const Json 
 			       ",\"num_blocks\":" + std::to_string(ranges[2 * k + 1]) + "}";
 		}
 		return result(id, out + "],\"truncated\":" + (res.truncated ? "true" : "false") + "}");
+	}
+	if (method == "replace_mirror_replica") {
+		/* move an imported replica to the store behind `remote_replica` (a base64 handle, as export_bdev_store gives it):
+		 * replica 0 is copied into it with the sessions held, and the old exporter may delete its bdev afterwards */
+		int32_t rep = 0;
+		std::string h;
+		if (!decode(params, {{"name", Json::Str, false, &a}, {"replica", Json::Num, false, &b}, {"remote_replica", Json::Str, false, &c}}) ||
+		    !to_i32(b, &rep) || !base64_decode(c->raw, &h) || h.size() != OIMGPU_IPC_HANDLE_BYTES)
+			return bad;
+		int rc = oimgpu_bdev_mirror_replace_remote(a->raw.c_str(), rep, h.data());
+		if (rc < 0) return error(id, E_INVALID_PARAMS, strerr(rc));
+		return result(id, "true");
 	}
 	if (method == "delete_bdev") {
 		if (!decode(params, {{"name", Json::Str, false, &a}})) return bad;

@@ -67,6 +67,7 @@ SYMBOLS = [
     ("oimgpu_bdev_create_mirror_uuid", _I, [C.c_char_p, C.c_char_p, _U64, _U32, C.POINTER(C.c_int), _I, C.c_char_p, C.c_size_t]),
     ("oimgpu_bdev_create_mirror_remote_uuid", _I, [C.c_char_p, C.c_char_p, _U64, _U32, _I, _VP, _I, C.c_char_p, C.c_size_t]),
     ("oimgpu_bdev_replica_info", _I, [C.c_char_p, _I, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    ("oimgpu_bdev_mirror_replace_remote", _I, [C.c_char_p, _I, _VP]),
     ("oimgpu_bdev_digest", _I, [C.c_char_p, _I, _U64, _U64, C.POINTER(C.c_uint64)]),
     ("oimgpu_digest_device", _I, [_I, _VP, _U64, C.POINTER(C.c_uint64)]),
     ("oimgpu_bdev_mirror_check", _I, [C.c_char_p, _U64, _U64, _I, _VP, _U32, _VP]),
@@ -223,6 +224,15 @@ def construct_mirror_bdev_remote(num_blocks: int, block_size: int, device: int, 
     _chk(load().oimgpu_bdev_create_mirror_remote(_b(name), num_blocks, block_size, device, blob, len(peer_handles), out, 64),
          "construct_mirror_bdev_remote")
     return out.value.decode()
+
+
+def mirror_replace_remote(name: str, replica: int, handle: bytes) -> None:
+    """move replica `replica` (>= 1) of a mirror built from remote replicas to the store behind `handle`, copying
+    replica 0 into it with the sessions held (include/oimgpu.h oimgpu_bdev_mirror_replace_remote)"""
+    if len(handle) != IPC_HANDLE_BYTES:
+        raise ValueError(f"an IPC handle is {IPC_HANDLE_BYTES} bytes, not {len(handle)}")
+    blob = C.create_string_buffer(bytes(handle), IPC_HANDLE_BYTES)
+    _chk(load().oimgpu_bdev_mirror_replace_remote(_b(name), replica, blob), "mirror_replace_remote")
 
 
 def bdev_digest(name: str, replica: int = 0, offset: int = 0, nbytes: int | None = None) -> tuple[int, int]:
