@@ -85,17 +85,17 @@ extern "C" int oimgpu_bio_chan_open(const char *bdev_name, oimgpu_bio_chan **out
 	if (!g.inited || g.control_only) return -ENODEV;
 	Bdev *b = find_bdev_locked(bdev_name);
 	if (!b) return -ENODEV;
-	if (b->stores.size() != 1) return -ENOTSUP;	/* mirrored: the fan-out to replicas is not done here */
+	if (b->replicas.size() != 1) return -ENOTSUP;	/* mirrored: the fan-out to replicas is not done here */
 	auto c = std::make_unique<oimgpu_bio_chan>();
 	c->bdev = b->name;
-	c->device = b->devices[0];
+	c->device = b->replicas[0].device;
 	c->sm_count = g.devices[find_device_slot(c->device)].sm_count;
-	c->store = b->stores[0];
+	c->store = b->replicas[0].store;
 	c->num_blocks = b->num_blocks;
 	c->block_size = b->block_size;
 	CU_OK(cudaSetDevice(c->device));
 	CU_OK(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
-	b->open_luns++;		/* pins the bdev: oimgpu_bdev_delete returns -EBUSY */
+	open_bdev_locked(*b);	/* oimgpu_bdev_delete returns -EBUSY while the channel is open */
 	*out = c.release();
 	return 0;
 }
@@ -117,7 +117,7 @@ extern "C" int oimgpu_bio_chan_close(oimgpu_bio_chan *c)
 			for (auto &st : c->staging) if (st.h) cudaFreeHost(st.h);
 			for (BioSeg *h : c->retired_staging) cudaFreeHost(h);
 		}
-		if (Bdev *b = find_bdev_locked(c->bdev.c_str())) b->open_luns--;
+		close_bdev_locked(c->bdev);
 	}
 	delete c;
 	return 0;

@@ -68,14 +68,32 @@ static void copy_str(char *dst, size_t cap, const std::string &s)
 
 /* ---- lifecycle ------------------------------------------------------------------------------- */
 
-static void release_store(Bdev &b, size_t r)
+static void release_store(const Replica &r)
 {
-	cudaSetDevice(b.devices[r]);
-	if (b.imported[r]) cudaIpcCloseMemHandle(b.stores[r]);
-	else cudaFree(b.stores[r]);
+	cudaSetDevice(r.device);
+	if (r.imported) cudaIpcCloseMemHandle(r.store);
+	else cudaFree(r.store);
 	(void)cudaGetLastError();
 }
 
+/* Take a bdev apart once nothing uses it: own stores are freed (their bytes given back to their GPU's count, which
+ * places later bdevs), imported ones closed, the histogram freed and the name unregistered.  The pollers of each
+ * replica's GPU are parked around its release. */
+static void drop_bdev_locked(Bdev *b)
+{
+	if (!g.control_only) {
+		for (const Replica &r : b->replicas) {
+			{
+				ParkedPollers parked(r.device);
+				release_store(r);
+			}
+			if (!r.imported) g.devices[find_device_slot(r.device)].bytes_allocated -= b->num_blocks * (uint64_t)b->block_size;
+		}
+		if (b->hist) { cudaSetDevice(b->replicas[0].device); cudaFree(b->hist); }
+	}
+	g.bdev_order.erase(std::remove(g.bdev_order.begin(), g.bdev_order.end(), b->name), g.bdev_order.end());
+	g.bdevs.erase(g.bdevs.find(b->name));
+}
 
 extern "C" int oimgpu_abi_version(void) { return OIMGPU_ABI_VERSION; }
 
@@ -143,14 +161,9 @@ extern "C" void oimgpu_fini(void)
 	std::lock_guard<std::mutex> lk(g.mu);
 	if (!g.inited) return;
 	if (!g.control_only) unpin_all_host_ranges();
-	for (auto &kv : g.bdevs) {
-		for (size_t r = 0; r < kv.second->stores.size() && !g.control_only; r++) release_store(*kv.second, r);
-		if (kv.second->hist && !g.control_only) { cudaSetDevice(kv.second->devices[0]); cudaFree(kv.second->hist); }
-	}
+	while (!g.bdevs.empty()) drop_bdev_locked(g.bdevs.begin()->second.get());
 	g.control_only = false;
-	g.bdevs.clear();
 	g.ctrlrs.clear();
-	g.bdev_order.clear();
 	g.ctrlr_order.clear();
 	memset(g.scsi_slot_used, 0, sizeof(g.scsi_slot_used));
 	for (auto &d : g.devices) {
@@ -202,40 +215,37 @@ static int alloc_store(int ordinal, uint64_t bytes, uint8_t **out)
 	return 0;
 }
 
+/* A bdev with an own store on each of `devs`, named `name` or, without one, `prefix` + `counter` (the counter advances
+ * only when such a bdev is made).  *out: the registered bdev. */
 static int create_bdev_locked(const char *name, const char *uuid, uint64_t num_blocks, uint32_t block_size,
-			      const std::vector<int> &devs, const char *product, const std::string &auto_name,
-			      char *name_out, size_t name_cap)
+			      const std::vector<int> &devs, const char *product, const char *prefix, int &counter, Bdev **out)
 {
 	if (!g.inited) return -ENODEV;
 	/* create_malloc_disk: "Disk must be more than 0 blocks" (bdev_malloc.c:384-387); block size must
 	 * be a positive multiple the SCSI layer can divide 4 MiB by */
 	if (num_blocks == 0 || block_size == 0 || block_size > OIMGPU_MAX_XFER_BYTES) return -EINVAL;
 	if (uuid && !uuid_valid(uuid)) return -EINVAL;
-	std::string nm = name && name[0] ? name : auto_name;
+	const bool auto_named = !(name && name[0]);
+	const std::string nm = auto_named ? prefix + std::to_string(counter) : name;
 	if (g.bdevs.count(nm)) return -EEXIST;	/* spdk_bdev_register: name already in use */
-	auto b = std::make_unique<Bdev>();
+	Bdev *b = (g.bdevs[nm] = std::make_unique<Bdev>()).get();
+	g.bdev_order.push_back(nm);
 	b->name = nm;
 	b->product = product;
 	b->uuid = uuid ? uuid : random_uuid();
 	b->num_blocks = num_blocks;
 	b->block_size = block_size;
 	for (int d : devs) {
-		uint8_t *p = nullptr;
-		int rc = alloc_store(d, num_blocks * (uint64_t)block_size, &p);
-		if (rc != 0) {
-			for (size_t r = 0; r < b->stores.size(); r++) {
-				cudaSetDevice(b->devices[r]);
-				cudaFree(b->stores[r]);
-			}
+		Replica r;
+		r.device = d;
+		if (int rc = alloc_store(d, num_blocks * (uint64_t)block_size, &r.store)) {
+			drop_bdev_locked(b);
 			return rc;
 		}
-		b->devices.push_back(d);
-		b->stores.push_back(p);
-		b->imported.push_back(0);
+		b->replicas.push_back(r);
 	}
-	copy_str(name_out, name_cap, nm);
-	g.bdevs[nm] = std::move(b);
-	g.bdev_order.push_back(nm);
+	if (auto_named) counter++;
+	*out = b;
 	return 0;
 }
 
@@ -246,10 +256,9 @@ extern "C" int oimgpu_bdev_create_malloc(const char *name, const char *uuid, uin
 	if (!g.inited) return -ENODEV;
 	int d = pick_device(device);
 	if (d < 0) return -EINVAL;
-	std::string auto_name;
-	if (!(name && name[0])) auto_name = "Malloc" + std::to_string(g.malloc_disk_count);
-	int rc = create_bdev_locked(name, uuid, num_blocks, block_size, {d}, "Malloc disk", auto_name, name_out, name_cap);
-	if (rc == 0 && !(name && name[0])) g.malloc_disk_count++;
+	Bdev *b = nullptr;
+	int rc = create_bdev_locked(name, uuid, num_blocks, block_size, {d}, "Malloc disk", "Malloc", g.malloc_disk_count, &b);
+	if (rc == 0) copy_str(name_out, name_cap, b->name);
 	return rc;
 }
 
@@ -265,18 +274,15 @@ extern "C" int oimgpu_bdev_create_rbd(const char *name, const char *pool_name, c
 	if (size_bytes == 0 || size_bytes % block_size) return -EINVAL;
 	int d = pick_device(device);
 	if (d < 0) return -EINVAL;
-	std::string auto_name;
-	if (!(name && name[0])) auto_name = "Ceph" + std::to_string(g.rbd_count);	/* bdev_rbd.c:732 */
+	Bdev *b = nullptr;
 	int rc = create_bdev_locked(name, nullptr, size_bytes / block_size, block_size, {d}, "Ceph Rbd Disk",
-				    auto_name, name_out, name_cap);
-	if (rc == 0 && !(name && name[0])) g.rbd_count++;
-	if (rc == 0) {
-		Bdev &b = *g.bdevs[name && name[0] ? std::string(name) : auto_name];
-		b.pool_name = pool_name;
-		b.rbd_name = rbd_name;
-		b.user_id = user_id ? user_id : "";
-	}
-	return rc;
+				    "Ceph", g.rbd_count, &b);	/* bdev_rbd.c:732 */
+	if (rc) return rc;
+	b->pool_name = pool_name;
+	b->rbd_name = rbd_name;
+	b->user_id = user_id ? user_id : "";
+	copy_str(name_out, name_cap, b->name);
+	return 0;
 }
 
 extern "C" int oimgpu_bdev_create_mirror(const char *name, uint64_t num_blocks, uint32_t block_size,
@@ -307,10 +313,9 @@ extern "C" int oimgpu_bdev_create_mirror_uuid(const char *name, const char *uuid
 		int can = 0;
 		if (devs[0] != devs[r] && (cudaDeviceCanAccessPeer(&can, devs[0], devs[r]) != cudaSuccess || !can)) return -ENOTSUP;
 	}
-	std::string auto_name;
-	if (!(name && name[0])) auto_name = "Mirror" + std::to_string(g.malloc_disk_count);
-	int rc = create_bdev_locked(name, uuid, num_blocks, block_size, devs, "Malloc disk", auto_name, name_out, name_cap);
-	if (rc == 0 && !(name && name[0])) g.malloc_disk_count++;
+	Bdev *b = nullptr;
+	int rc = create_bdev_locked(name, uuid, num_blocks, block_size, devs, "Malloc disk", "Mirror", g.malloc_disk_count, &b);
+	if (rc == 0) copy_str(name_out, name_cap, b->name);
 	return rc;
 }
 
@@ -322,10 +327,10 @@ extern "C" int oimgpu_bdev_export_store(const char *name, int replica, void *han
 	if (!handle_out) return -EINVAL;
 	Bdev *b = find_bdev_locked(name);
 	if (!b) return -ENODEV;
-	if (replica < 0 || replica >= (int)b->stores.size() || b->imported[replica]) return -EINVAL;
-	CU_OK(cudaSetDevice(b->devices[replica]));
+	if (replica < 0 || replica >= (int)b->replicas.size() || b->replicas[replica].imported) return -EINVAL;
+	CU_OK(cudaSetDevice(b->replicas[replica].device));
 	cudaIpcMemHandle_t h;
-	CU_OK(cudaIpcGetMemHandle(&h, b->stores[replica]));
+	CU_OK(cudaIpcGetMemHandle(&h, b->replicas[replica].store));
 	memcpy(handle_out, &h, sizeof(h));
 	return 0;
 }
@@ -346,13 +351,9 @@ extern "C" int oimgpu_bdev_create_mirror_remote_uuid(const char *name, const cha
 	if (!peer_handles || npeers < 1 || npeers >= kMaxReplicas) return -EINVAL;
 	int d = pick_device(device);
 	if (d < 0) return -EINVAL;
-	std::string auto_name;
-	if (!(name && name[0])) auto_name = "Mirror" + std::to_string(g.malloc_disk_count);
-	char nm[64];
-	int rc = create_bdev_locked(name, uuid, num_blocks, block_size, {d}, "Malloc disk", auto_name, nm, sizeof(nm));
+	Bdev *b = nullptr;
+	int rc = create_bdev_locked(name, uuid, num_blocks, block_size, {d}, "Malloc disk", "Mirror", g.malloc_disk_count, &b);
 	if (rc) return rc;
-	if (!(name && name[0])) g.malloc_disk_count++;
-	Bdev &b = *g.bdevs[nm];
 	CU_OK(cudaSetDevice(d));
 	for (int r = 0; r < npeers; r++) {
 		cudaIpcMemHandle_t h;
@@ -362,17 +363,12 @@ extern "C" int oimgpu_bdev_create_mirror_remote_uuid(const char *name, const cha
 		if (e != cudaSuccess) {
 			fprintf(stderr, "oimgpu: cudaIpcOpenMemHandle failed: %s\n", cudaGetErrorString(e));
 			(void)cudaGetLastError();
-			for (size_t k = 0; k < b.stores.size(); k++) release_store(b, k);
-			g.bdev_order.erase(std::remove(g.bdev_order.begin(), g.bdev_order.end(), std::string(nm)), g.bdev_order.end());
-			g.bdevs.erase(nm);
+			drop_bdev_locked(b);
 			return -EIO;
 		}
-		b.devices.push_back(d);
-		b.stores.push_back((uint8_t *)p);
-		b.imported.push_back(1);
-		b.ipc_handles.emplace_back((const char *)&h, sizeof(h));
+		b->replicas.push_back({d, (uint8_t *)p, true, std::string((const char *)&h, sizeof(h))});
 	}
-	copy_str(name_out, name_cap, nm);
+	copy_str(name_out, name_cap, b->name);
 	return 0;
 }
 
@@ -382,9 +378,9 @@ extern "C" int oimgpu_bdev_replica_info(const char *name, int replica, int *devi
 	if (!g.inited) return -ENODEV;
 	Bdev *b = find_bdev_locked(name);
 	if (!b) return -ENODEV;
-	if (replica < 0 || replica >= (int)b->stores.size()) return -EINVAL;
-	if (device) *device = b->devices[replica];
-	if (imported) *imported = b->imported[replica];
+	if (replica < 0 || replica >= (int)b->replicas.size()) return -EINVAL;
+	if (device) *device = b->replicas[replica].device;
+	if (imported) *imported = b->replicas[replica].imported;
 	return 0;
 }
 
@@ -398,24 +394,23 @@ extern "C" int oimgpu_bdev_mirror_replace_remote(const char *name, int replica, 
 	Bdev *b = find_bdev_locked(name);
 	if (!b) return -ENODEV;
 	/* only a mirror built from handles: the configuration dump can then name the new store */
-	if (b->stores.size() < 2) return -ENOTSUP;
-	for (size_t r = 1; r < b->stores.size(); r++) {
-		if (!b->imported[r]) return -ENOTSUP;
+	if (b->replicas.size() < 2) return -ENOTSUP;
+	for (size_t r = 1; r < b->replicas.size(); r++) {
+		if (!b->replicas[r].imported) return -ENOTSUP;
 	}
-	if (replica < 1 || replica >= (int)b->stores.size()) return -EINVAL;
+	if (replica < 1 || replica >= (int)b->replicas.size()) return -EINVAL;
 	/* by its bytes, before it is opened: what the driver does with a handle this process holds open is not ours to rely on */
 	const std::string h((const char *)handle, OIMGPU_IPC_HANDLE_BYTES);
-	if (std::find(b->ipc_handles.begin(), b->ipc_handles.end(), h) != b->ipc_handles.end()) return -EINVAL;
+	for (const Replica &r : b->replicas) {
+		if (r.ipc_handle == h) return -EINVAL;
+	}
 	if (b->nbd_exports) return -EBUSY;	/* an NBD export moves payload with no point at which it could be paused */
 
 	/* as oimgpu_bdev_mirror_check: every session that reaches the bdev, and every session on replica 0's GPU, held
 	 * and drained for the whole call */
-	const int dev0 = b->devices[0];
+	const int dev0 = b->replicas[0].device;
 	ParkedPollers held(dev0, b->name);
-	for (const auto &p : held.parked) {
-		CU_OK(cudaSetDevice(p.L->device));
-		CU_OK(cudaStreamSynchronize(p.L->stream));
-	}
+	if (int rc = held.drain()) return rc;
 	CU_OK(cudaSetDevice(dev0));
 	cudaIpcMemHandle_t ih;
 	memcpy(&ih, handle, sizeof(ih));
@@ -426,7 +421,8 @@ extern "C" int oimgpu_bdev_mirror_replace_remote(const char *name, int replica, 
 		(void)cudaGetLastError();
 		return e == cudaErrorPeerAccessUnsupported ? -ENOTSUP : -EIO;
 	}
-	uint8_t *fresh = (uint8_t *)p, *old = b->stores[replica];
+	Replica &rep = b->replicas[replica];
+	uint8_t *fresh = (uint8_t *)p, *old = rep.store;
 	auto drop = [&](int rc) {
 		cudaSetDevice(dev0);
 		cudaIpcCloseMemHandle(fresh);
@@ -438,21 +434,22 @@ extern "C" int oimgpu_bdev_mirror_replace_remote(const char *name, int replica, 
 	if (!device_reachable(dev0, at.device)) return drop(-ENOTSUP);
 	const Device &dev = g.devices[find_device_slot(dev0)];
 	e = cudaSetDevice(dev0);
-	if (e == cudaSuccess) e = launch_copy(dev.util, dev.sm_count, fresh, b->stores[0], b->num_blocks * (uint64_t)b->block_size);
+	if (e == cudaSuccess) e = launch_copy(dev.util, dev.sm_count, fresh, b->replicas[0].store, b->num_blocks * (uint64_t)b->block_size);
 	if (e == cudaSuccess) e = cudaStreamSynchronize(dev.util);
 	if (e != cudaSuccess) {
 		fprintf(stderr, "oimgpu: copy of %s replica 0 to its new replica %d failed: %s\n", b->name.c_str(), replica,
 			cudaGetErrorString(e));
 		return drop(-EIO);
 	}
-	int rc = publish_replica_locked(b->name, replica, fresh);
+	const size_t field = offsetof(LunCtx, store) + sizeof(uint8_t *) * replica;
+	int rc = publish_ctx_locked(b->name, field, &fresh, sizeof(fresh));
 	if (rc) {
-		publish_replica_locked(b->name, replica, old);
+		publish_ctx_locked(b->name, field, &old, sizeof(old));
 		return drop(rc);
 	}
-	release_store(*b, (size_t)replica);
-	b->stores[replica] = fresh;
-	b->ipc_handles[replica - 1] = h;	/* replicas 1.. are all imported: handle k is replica k + 1's */
+	release_store(rep);
+	rep.store = fresh;
+	rep.ipc_handle = h;
 	return 0;
 }
 
@@ -504,12 +501,12 @@ extern "C" int oimgpu_bdev_digest(const char *name, int replica, uint64_t offset
 	if (!g.inited || g.control_only) return -ENODEV;
 	Bdev *b = find_bdev_locked(name);
 	if (!b) return -ENODEV;
-	if (replica < 0 || replica >= (int)b->stores.size()) return -EINVAL;
+	if (replica < 0 || replica >= (int)b->replicas.size()) return -EINVAL;
 	const uint64_t size = b->num_blocks * (uint64_t)b->block_size;
 	if (offset > size || nbytes > size - offset || (offset & 7)) return -EINVAL;
 	int rc = sync_session_streams_locked();
 	if (rc) return rc;
-	return digest_locked(b->devices[replica], b->stores[replica] + offset, nbytes, out);
+	return digest_locked(b->replicas[replica].device, b->replicas[replica].store + offset, nbytes, out);
 }
 
 extern "C" int oimgpu_bdev_delete(const char *name)
@@ -518,15 +515,14 @@ extern "C" int oimgpu_bdev_delete(const char *name)
 	if (!g.inited) return -ENODEV;
 	Bdev *b = find_bdev_locked(name);
 	if (!b) return -ENODEV;
-	/* a session opened on exactly this device pins it; controller-wide sessions let go of it below */
+	/* the peer-target contexts of controller-wide sessions let go of it below, as its targets go; every other use (a
+	 * session opened on exactly this device, an NBD export, a bio channel) is checked BEFORE anything is taken apart: a
+	 * failed delete must leave the targets where they were */
 	int peer_refs = 0;
 	for (oimgpu_lun *L : g.handles) {
-		if (L->bdev == b->name) return -EBUSY;
-		for (int t = 0; t < OIMGPU_CTRLR_MAX_DEVS; t++) peer_refs += L->peer_bdev[t] == b->name;
+		for_each_ctx(L, [&](const std::string &name, LunCtx *, LunCtx *h) { peer_refs += !h && name == b->name; return 0; });
 	}
-	/* every other pin (an NBD export, oimgpu_nbd_serve) is checked BEFORE anything is taken apart: a failed
-	 * delete must leave the targets where they were */
-	if (b->open_luns > peer_refs) return -EBUSY;
+	if (b->opens > peer_refs) return -EBUSY;
 	/* spdk_bdev_unregister hot-removes the SCSI LUNs built on the bdev (lun.c:213-260): the targets go */
 	for (auto &kv : g.ctrlrs) {
 		bool touched = false;
@@ -539,38 +535,8 @@ extern "C" int oimgpu_bdev_delete(const char *name)
 		}
 		if (touched && !g.control_only) refresh_ctrlr_sessions_locked(kv.first);
 	}
-	if (b->open_luns) return -EBUSY;
-	g.bdev_order.erase(std::remove(g.bdev_order.begin(), g.bdev_order.end(), b->name), g.bdev_order.end());
-	for (size_t r = 0; r < b->stores.size() && !g.control_only; r++) {
-		const bool own = !b->imported[r];
-		{
-			ParkedPollers parked(b->devices[r]);
-			release_store(*b, r);
-		}
-		if (own) g.devices[find_device_slot(b->devices[r])].bytes_allocated -= b->num_blocks * (uint64_t)b->block_size;
-	}
-	if (b->hist) { cudaSetDevice(b->devices[0]); cudaFree(b->hist); }
-	g.bdevs.erase(g.bdevs.find(b->name));
-	return 0;
-}
-
-/* every open session's device-resident view of the bdev learns where its histogram is (or that it is gone) */
-static int publish_hist_locked(const std::string &name, unsigned long long *hist)
-{
-	for (oimgpu_lun *L : g.handles) {
-		std::lock_guard<std::recursive_mutex> hl(L->mu);
-		CU_OK(cudaSetDevice(L->device));
-		if (L->bdev == name) {
-			L->h_ctx.hist = hist;
-			CU_OK(cudaMemcpyAsync((uint8_t *)L->d_ctx + offsetof(LunCtx, hist), &L->h_ctx.hist, sizeof(hist), cudaMemcpyHostToDevice, L->copy_stream));
-			CU_OK(cudaStreamSynchronize(L->copy_stream));
-		}
-		for (int t = 0; t < OIMGPU_CTRLR_MAX_DEVS; t++) {
-			if (L->peer_bdev[t] != name || !L->d_peer[t]) continue;
-			CU_OK(cudaMemcpyAsync((uint8_t *)L->d_peer[t] + offsetof(LunCtx, hist), &hist, sizeof(hist), cudaMemcpyHostToDevice, L->copy_stream));
-			CU_OK(cudaStreamSynchronize(L->copy_stream));
-		}
-	}
+	if (b->opens) return -EBUSY;
+	drop_bdev_locked(b);
 	return 0;
 }
 
@@ -583,8 +549,10 @@ extern "C" int oimgpu_bdev_histogram_enable(const char *name, int enable)
 	Bdev *b = find_bdev_locked(name);
 	if (!b) return -ENODEV;
 	if (g.control_only) { b->hist = enable ? (unsigned long long *)1 : nullptr; return 0; }
-	CU_OK(cudaSetDevice(b->devices[0]));
-	cudaStream_t st = g.devices[find_device_slot(b->devices[0])].util;
+	const int dev0 = b->replicas[0].device;
+	CU_OK(cudaSetDevice(dev0));
+	cudaStream_t st = g.devices[find_device_slot(dev0)].util;
+	/* every open session's device-resident view of the bdev learns where its histogram is (or that it is gone) */
 	if (enable) {
 		if (!b->hist) {
 			unsigned long long *h = nullptr;
@@ -593,16 +561,17 @@ extern "C" int oimgpu_bdev_histogram_enable(const char *name, int enable)
 		}
 		CU_OK(cudaMemsetAsync(b->hist, 0, sizeof(unsigned long long) * kHistBuckets, st));
 		CU_OK(cudaStreamSynchronize(st));
-		return publish_hist_locked(b->name, b->hist);
+		return publish_ctx_locked(b->name, offsetof(LunCtx, hist), &b->hist, sizeof(b->hist));
 	}
 	if (b->hist) {
-		int rc = publish_hist_locked(b->name, nullptr);
+		unsigned long long *none = nullptr;
+		int rc = publish_ctx_locked(b->name, offsetof(LunCtx, hist), &none, sizeof(none));
 		if (rc) return rc;
 		/* kernels already launched may still tally: everything in flight first, resident pollers parked */
 		{
 			ParkedPollers parked(-1);
 			(void)sync_session_streams_locked();
-			cudaSetDevice(b->devices[0]);
+			cudaSetDevice(dev0);
 			cudaFree(b->hist);
 		}
 		b->hist = nullptr;
@@ -620,10 +589,10 @@ extern "C" int oimgpu_bdev_histogram_get(const char *name, uint64_t *buckets)
 	if (!b) return -ENODEV;
 	if (!buckets) return -EINVAL;
 	memset(buckets, 0, sizeof(uint64_t) * kHistBuckets);
-	if (!b->hist) return b->open_luns > 0 ? -EFAULT : 0;	/* I/O channels exist while a session runs (spdk_scsi_dev_allocate_io_channels) */
+	if (!b->hist) return b->opens > 0 ? -EFAULT : 0;	/* I/O channels exist while a session runs (spdk_scsi_dev_allocate_io_channels) */
 	if (g.control_only) return 0;
-	CU_OK(cudaSetDevice(b->devices[0]));
-	cudaStream_t st = g.devices[find_device_slot(b->devices[0])].util;
+	CU_OK(cudaSetDevice(b->replicas[0].device));
+	cudaStream_t st = g.devices[find_device_slot(b->replicas[0].device)].util;
 	CU_OK(cudaMemcpyAsync(buckets, b->hist, sizeof(uint64_t) * kHistBuckets, cudaMemcpyDeviceToHost, st));
 	CU_OK(cudaStreamSynchronize(st));
 	return 0;
@@ -638,9 +607,9 @@ static void fill_bdev_info(const Bdev &b, oimgpu_bdev_info *o)
 	o->num_blocks = b.num_blocks;
 	o->block_size = b.block_size;
 	o->claimed = 0;	/* SCSI LUNs open the bdev without claiming it (lun.c:342): get_bdevs says false */
-	o->device = b.devices[0];
-	o->replicas = (uint32_t)b.stores.size();
-	o->device_ptr = (uint64_t)(uintptr_t)b.stores[0];
+	o->device = b.replicas[0].device;
+	o->replicas = (uint32_t)b.replicas.size();
+	o->device_ptr = (uint64_t)(uintptr_t)b.replicas[0].store;
 }
 
 extern "C" int oimgpu_bdev_get(const char *name, oimgpu_bdev_info *out)
@@ -658,7 +627,7 @@ extern "C" int oimgpu_bdev_list(oimgpu_bdev_info *out, int max)
 	std::lock_guard<std::mutex> lk(g.mu);
 	int n = 0;
 	for (auto &nm : g.bdev_order) {
-		if (out && n < max) fill_bdev_info(*g.bdevs[nm], &out[n]);
+		if (out && n < max) fill_bdev_info(*find_bdev_locked(nm.c_str()), &out[n]);
 		n++;
 	}
 	return n;
@@ -670,16 +639,17 @@ static int raw_access(const char *name, int replica, uint64_t offset, void *host
 	if (!g.inited || g.control_only) return -ENODEV;
 	Bdev *b = find_bdev_locked(name);
 	if (!b) return -ENODEV;
-	if (replica < 0 || replica >= (int)b->stores.size()) return -EINVAL;
+	if (replica < 0 || replica >= (int)b->replicas.size()) return -EINVAL;
+	const Replica &r = b->replicas[replica];
 	uint64_t size = b->num_blocks * (uint64_t)b->block_size;
 	if (offset > size || len > size - offset) return -EINVAL;
-	CU_OK(cudaSetDevice(b->devices[replica]));
+	CU_OK(cudaSetDevice(r.device));
 	int rc = sync_session_streams_locked();
 	if (rc) return rc;
-	CU_OK(cudaSetDevice(b->devices[replica]));
-	cudaStream_t st = g.devices[find_device_slot(b->devices[replica])].util;
-	if (write) CU_OK(cudaMemcpyAsync(b->stores[replica] + offset, host, len, cudaMemcpyHostToDevice, st));
-	else CU_OK(cudaMemcpyAsync(host, b->stores[replica] + offset, len, cudaMemcpyDeviceToHost, st));
+	CU_OK(cudaSetDevice(r.device));
+	cudaStream_t st = g.devices[find_device_slot(r.device)].util;
+	if (write) CU_OK(cudaMemcpyAsync(r.store + offset, host, len, cudaMemcpyHostToDevice, st));
+	else CU_OK(cudaMemcpyAsync(host, r.store + offset, len, cudaMemcpyDeviceToHost, st));
 	CU_OK(cudaStreamSynchronize(st));
 	return 0;
 }
@@ -751,6 +721,14 @@ Bdev *oimgpu::find_bdev_locked(const char *name)
 	return it == g.bdevs.end() ? nullptr : it->second.get();
 }
 
+void oimgpu::open_bdev_locked(Bdev &b) { b.opens++; }
+
+void oimgpu::close_bdev_locked(const std::string &name)
+{
+	Bdev *b = find_bdev_locked(name.c_str());
+	if (b && b->opens > 0) b->opens--;
+}
+
 /* vhost -S <dir> (S/lib/vhost/vhost.c:1185-1205): controller sockets live at <dir>/<name> */
 extern "C" int oimgpu_set_socket_dir(const char *dir, const char *app_core_mask)
 {
@@ -812,15 +790,13 @@ extern "C" int oimgpu_vhost_scsi_add_lun(const char *ctrlr, int scsi_target_num,
 	}
 	if (!bdev_name) return -EINVAL;
 	if (!c->targets[scsi_target_num].empty()) return -EEXIST;
-	Bdev *b = find_bdev_locked(bdev_name);
-	if (!b) return -EINVAL;	/* spdk_scsi_dev_construct failed */
+	if (!find_bdev_locked(bdev_name)) return -EINVAL;	/* spdk_scsi_dev_construct failed */
 	int slot = 0;
 	while (slot < 1024 && g.scsi_slot_used[slot]) slot++;
 	if (slot == 1024) return -EINVAL;	/* spdk_scsi_dev_construct: no free device slot */
 	g.scsi_slot_used[slot] = true;
 	c->scsi_id[scsi_target_num] = slot;
 	c->targets[scsi_target_num] = bdev_name;
-	b->claimed++;
 	if (!g.control_only) refresh_ctrlr_sessions_locked(c->name);	/* hot-plug into running sessions */
 	return scsi_target_num;
 }
@@ -833,8 +809,6 @@ extern "C" int oimgpu_vhost_scsi_remove_target(const char *ctrlr, int scsi_targe
 	if (!c) return -ENODEV;
 	if (scsi_target_num < 0 || scsi_target_num >= OIMGPU_CTRLR_MAX_DEVS) return -EINVAL;
 	if (c->targets[scsi_target_num].empty()) return -ENODEV;
-	Bdev *b = find_bdev_locked(c->targets[scsi_target_num].c_str());
-	if (b && b->claimed > 0) b->claimed--;
 	/* a session opened on exactly this target keeps serving it until it is closed (the reference
 	 * defers the removal until the session has no task in flight, vhost_scsi.c:236-289); for every
 	 * other session of the controller the target disappears now */
@@ -914,24 +888,23 @@ extern "C" long oimgpu_config_json(const char *subsystem, char *buf, size_t cap)
 	if (sub == "bdev") {
 		out += "{\"method\":\"set_bdev_options\",\"params\":{\"bdev_io_pool_size\":65536,\"bdev_io_cache_size\":256}}";
 		for (auto &nm : g.bdev_order) {
-			const Bdev &b = *g.bdevs[nm];
+			const Bdev &b = *find_bdev_locked(nm.c_str());
 			if (b.product == "Ceph Rbd Disk") {
 				out += ",{\"method\":\"construct_rbd_bdev\",\"params\":{\"name\":" + json_escape(b.name) + ",\"pool_name\":" +
 				       json_escape(b.pool_name) + ",\"rbd_name\":" + json_escape(b.rbd_name) + ",\"block_size\":" + std::to_string(b.block_size);
 				if (!b.user_id.empty()) out += ",\"user_id\":" + json_escape(b.user_id);
 				out += "}}";
-			} else if (b.stores.size() > 1) {
+			} else if (b.replicas.size() > 1) {
 				/* a mirror: in-process replicas are placed again by the rule, imported ones opened again from their
 				 * handles (which stay valid while the exporting process keeps its bdev) */
 				out += ",{\"method\":\"construct_mirror_bdev\",\"params\":{\"name\":" + json_escape(b.name) + ",\"num_blocks\":" +
 				       std::to_string(b.num_blocks) + ",\"block_size\":" + std::to_string(b.block_size) + ",\"uuid\":" + json_escape(b.uuid);
-				if (b.ipc_handles.empty()) {
-					out += ",\"replicas\":" + std::to_string(b.stores.size()) + "}}";
-				} else {
-					out += ",\"remote_replicas\":[";
-					for (size_t k = 0; k < b.ipc_handles.size(); k++) out += (k ? ",\"" : "\"") + base64(b.ipc_handles[k]) + "\"";
-					out += "]}}";
+				std::string remote;
+				for (const Replica &r : b.replicas) {
+					if (r.imported) remote += (remote.empty() ? "\"" : ",\"") + base64(r.ipc_handle) + "\"";
 				}
+				if (remote.empty()) out += ",\"replicas\":" + std::to_string(b.replicas.size()) + "}}";
+				else out += ",\"remote_replicas\":[" + remote + "]}}";
 			} else {
 				out += ",{\"method\":\"construct_malloc_bdev\",\"params\":{\"name\":" + json_escape(b.name) + ",\"num_blocks\":" +
 				       std::to_string(b.num_blocks) + ",\"block_size\":" + std::to_string(b.block_size) + ",\"uuid\":" + json_escape(b.uuid) + "}}";
@@ -1014,14 +987,12 @@ extern "C" int oimgpu_bdev_iostat(const char *name, oimgpu_iostat *out)
 	unsigned long long sum[12], v[12];
 	memcpy(sum, b->retired, sizeof(sum));
 	for (oimgpu_lun *L : g.handles) {
-		if (L->bdev == b->name && read_ctx_stats(L->device, L->d_ctx, v)) {
-			for (int k = 0; k < 12; k++) sum[k] += v[k];
-		}
-		for (int t = 0; t < OIMGPU_CTRLR_MAX_DEVS; t++) {
-			if (L->peer_bdev[t] == b->name && read_ctx_stats(L->device, L->d_peer[t], v)) {
+		for_each_ctx(L, [&](const std::string &bn, LunCtx *d, LunCtx *) {
+			if (bn == b->name && read_ctx_stats(L->device, d, v)) {
 				for (int k = 0; k < 12; k++) sum[k] += v[k];
 			}
-		}
+			return 0;
+		});
 	}
 	iostat_from_stats(sum, out);
 	return 0;

@@ -42,19 +42,22 @@ struct Device {
 	cudaStream_t util = nullptr;
 };
 
+struct Replica {
+	int device = -1;	/* the GPU the store lives on (an imported store: the GPU it is reached from) */
+	uint8_t *store = nullptr;
+	bool imported = false;	/* another process's store, opened from a CUDA IPC handle */
+	std::string ipc_handle;	/* the handle an imported store was opened from (config dump) */
+};
+
 struct Bdev {
 	std::string name, product, uuid;
 	std::string pool_name, rbd_name, user_id;	/* construct_rbd_bdev parameters, kept for the config dump */
 	uint64_t num_blocks = 0;
 	uint32_t block_size = 0;
-	int claimed = 0;	/* number of SCSI targets built on it */
-	int open_luns = 0;	/* oimgpu_lun handles */
-	int nbd_exports = 0;	/* oimgpu_nbd_serve calls serving it (also counted in open_luns) */
-	std::vector<int> devices;	/* replica r lives on devices[r] (an imported replica: the device it is reached from) */
-	std::vector<uint8_t *> stores;
-	std::vector<char> imported;	/* replica r is another process's store, opened from a CUDA IPC handle */
-	std::vector<std::string> ipc_handles;	/* the handles the imported replicas were opened from, in replica order (config dump) */
-	unsigned long long *hist = nullptr;	/* enable_bdev_histogram: kHistBuckets counters on devices[0] */
+	int opens = 0;		/* open_bdev_locked: session targets (own and peer), NBD exports, bio channels */
+	int nbd_exports = 0;	/* oimgpu_nbd_serve calls serving it (also counted in opens) */
+	std::vector<Replica> replicas;
+	unsigned long long *hist = nullptr;	/* enable_bdev_histogram: kHistBuckets counters on replica 0's GPU */
 	unsigned long long retired[12] = {};	/* counters of sessions that are gone (same layout as LunCtx::stats) */
 };
 
@@ -80,7 +83,6 @@ struct Registry {
 	int malloc_disk_count = 0;	/* bdev_malloc.c:93 */
 	int rbd_count = 0;
 	std::map<void *, size_t> registered;
-	int open_luns = 0;
 	std::vector<oimgpu_lun *> handles;	/* open data-path sessions: told about target hot-plug */
 };
 
@@ -116,11 +118,15 @@ int find_device_slot(int ordinal);
 bool device_reachable(int from, int to);
 std::string ctrlr_key(const char *ctrlr);
 Bdev *find_bdev_locked(const char *name);	/* nullptr: no such bdev */
+/* A use of a bdev by a session target (its own or a peer), an NBD export or a bio channel begins or ends.  A bdev in
+ * use is not deleted, and its disabled histogram reads as -EFAULT.  Caller holds g.mu. */
+void open_bdev_locked(Bdev &b);
+void close_bdev_locked(const std::string &name);	/* a bdev no longer registered is ignored */
 Ctrlr *find_ctrlr_locked(const char *ctrlr);	/* by ctrlr_key(ctrlr); nullptr: no such controller */
 bool read_ctx_stats(int device, const LunCtx *d_ctx, unsigned long long out[12]);
 void iostat_from_stats(const unsigned long long stats[12], oimgpu_iostat *out);
 void refresh_ctrlr_sessions_locked(const std::string &ctrlr);
-int publish_replica_locked(const std::string &bdev, int replica, uint8_t *store);	/* every LunCtx of the bdev */
+int publish_ctx_locked(const std::string &bdev, size_t offset, const void *value, size_t len);	/* every LunCtx of the bdev */
 cudaError_t launch_copy(cudaStream_t st, int sm_count, void *dst, const void *src, uint64_t nbytes);
 cudaError_t launch_fill(cudaStream_t st, int sm_count, void *dst, uint8_t fill, uint64_t nbytes);
 void unpin_all_host_ranges();	/* oimgpu_mem_ensure's registrations */
@@ -195,6 +201,21 @@ struct oimgpu_lun {
 	uint8_t *slab = nullptr;		/* the mapped pinned slab the per-queue rings are carved from */
 };
 
+/* Visit the device-resident LunCtxs of session L with the name of the bdev each serves: its own context (passed with
+ * its host copy h_ctx) and then the peer-target contexts of a controller-wide view (passed with nullptr).  Stops at
+ * the first visit that returns nonzero and returns that.  Caller holds g.mu, under which the peers change. */
+template <class Visit> int for_each_ctx(oimgpu_lun *L, Visit visit)
+{
+	if (!L->bdev.empty()) {
+		if (int rc = visit(L->bdev, L->d_ctx, &L->h_ctx)) return rc;
+	}
+	for (int t = 0; t < OIMGPU_CTRLR_MAX_DEVS; t++) {
+		if (L->peer_bdev[t].empty()) continue;
+		if (int rc = visit(L->peer_bdev[t], L->d_peer[t], (LunCtx *)nullptr)) return rc;
+	}
+	return 0;
+}
+
 /* cudaFree waits for the whole device, and a resident poller kernel never finishes on its own: park
  * the pollers of that GPU around a free and bring them back afterwards.  Every session of the GPU is
  * held (its mutex taken) for the duration, so that none can start a resident kernel in the window -
@@ -204,16 +225,24 @@ struct ParkedPollers {
 	/* device < 0: every GPU (pinned host memory is mapped into all of them) */
 	explicit ParkedPollers(int device, oimgpu_lun *except = nullptr)
 	{
-		park([&](const oimgpu_lun *L) { return L != except && (device < 0 || L->device == device); });
+		park([&](oimgpu_lun *L) { return L != except && (device < 0 || L->device == device); });
 	}
-	/* every session on GPU `device`, and every session that reaches bdev `bdev` (its own device or a peer target) */
+	/* every session on GPU `device`, and every session that reaches bdev `bdev` (its own target or a peer target) */
 	ParkedPollers(int device, const std::string &bdev)
 	{
-		park([&](const oimgpu_lun *L) {
-			if (L->device == device || L->bdev == bdev) return true;
-			for (const std::string &p : L->peer_bdev) if (p == bdev) return true;
-			return false;
+		park([&](oimgpu_lun *L) {
+			return L->device == device ||
+			       for_each_ctx(L, [&](const std::string &name, LunCtx *, LunCtx *) { return (int)(name == bdev); });
 		});
+	}
+	/* wait for everything the held sessions launched: with their pollers parked, nothing is added behind it */
+	int drain()
+	{
+		for (const Session &p : parked) {
+			CU_OK(cudaSetDevice(p.L->device));
+			CU_OK(cudaStreamSynchronize(p.L->stream));
+		}
+		return 0;
 	}
 	~ParkedPollers()
 	{

@@ -155,7 +155,7 @@ extern "C" int oimgpu_bdev_mirror_check(const char *name, uint64_t offset_blocks
 	if (!g.inited || g.control_only) return -ENODEV;
 	Bdev *b = find_bdev_locked(name);
 	if (!b) return -ENODEV;
-	if (b->stores.size() < 2) return -ENOTSUP;
+	if (b->replicas.size() < 2) return -ENOTSUP;
 	if (offset_blocks > b->num_blocks || num_blocks > b->num_blocks - offset_blocks) return -EINVAL;
 	/* an NBD export moves payload with no point at which it could be paused */
 	if (b->nbd_exports) return -EBUSY;
@@ -166,18 +166,15 @@ extern "C" int oimgpu_bdev_mirror_check(const char *name, uint64_t offset_blocks
 	/* Writers in this process are held for the whole call: their resident pollers are parked (and restarted when
 	 * `held` goes), and what they launched is waited for.  The sessions on replica 0's GPU are held too: a resident
 	 * poller there could keep the check's CTAs from being scheduled. */
-	const int dev0 = b->devices[0];
+	const int dev0 = b->replicas[0].device;
 	ParkedPollers held(dev0, b->name);
-	for (const auto &p : held.parked) {
-		CU_OK(cudaSetDevice(p.L->device));
-		CU_OK(cudaStreamSynchronize(p.L->stream));
-	}
+	if (int rc = held.drain()) return rc;
 	const Device &dev = g.devices[find_device_slot(dev0)];
 	CU_OK(cudaSetDevice(dev0));
 	MirrorRange a;
 	memset(&a, 0, sizeof(a));
-	for (size_t r = 0; r < b->stores.size(); r++) a.store[r] = b->stores[r];
-	a.nreplicas = (uint32_t)b->stores.size();
+	for (size_t r = 0; r < b->replicas.size(); r++) a.store[r] = b->replicas[r].store;
+	a.nreplicas = (uint32_t)b->replicas.size();
 	a.block_size = b->block_size;
 	a.first_block = offset_blocks;
 	a.num_blocks = num_blocks;

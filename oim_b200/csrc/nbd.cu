@@ -38,30 +38,26 @@ static bool write_full(int fd, const void *buf, size_t n)
  * Returns 0 on an orderly end (NBD_CMD_DISC or EOF), -EINVAL on a bad request magic, -errno otherwise. */
 extern "C" int oimgpu_nbd_serve(const char *bdev_name, int sock_fd)
 {
-	uint8_t *stores[kMaxReplicas] = {};
-	int devices[kMaxReplicas] = {};
-	int nrep = 0;
+	std::vector<Replica> reps;
 	uint64_t size = 0;
 	uint32_t bs = 0;
 	std::string name = bdev_name ? bdev_name : "";
 	{
 		std::lock_guard<std::mutex> lk(g.mu);
 		if (!g.inited || g.control_only) return -ENODEV;
-		Bdev *bp = find_bdev_locked(name.c_str());
-		if (!bp) return -ENODEV;
-		Bdev &b = *bp;
-		nrep = (int)b.stores.size();
-		for (int r = 0; r < nrep; r++) { stores[r] = b.stores[r]; devices[r] = b.devices[r]; }
-		size = b.num_blocks * (uint64_t)b.block_size;
-		bs = b.block_size;
-		b.open_luns++;		/* pins the bdev like a session does */
-		b.nbd_exports++;	/* and refuses a mirror check: this loop cannot be paused */
+		Bdev *b = find_bdev_locked(name.c_str());
+		if (!b) return -ENODEV;
+		reps = b->replicas;
+		size = b->num_blocks * (uint64_t)b->block_size;
+		bs = b->block_size;
+		open_bdev_locked(*b);	/* a use like a session's */
+		b->nbd_exports++;	/* and refuses a mirror check: this loop cannot be paused */
 	}
 	int rc = 0;
 	cudaStream_t st = nullptr;
 	uint8_t *bounce = nullptr;
 	size_t cap = 0;
-	cudaSetDevice(devices[0]);
+	cudaSetDevice(reps[0].device);
 	if (cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking) != cudaSuccess) rc = -EIO;
 	auto book = [&](int op, uint64_t bytes) {	/* get_bdevs_iostat counts these like any other bdev I/O */
 		std::lock_guard<std::mutex> lk(g.mu);
@@ -97,19 +93,19 @@ extern "C" int oimgpu_nbd_serve(const char *bdev_name, int sock_fd)
 		switch (type) {
 		case 0:		/* NBD_CMD_READ */
 			ok = range_ok;
-			if (ok && payload) e = cudaMemcpyAsync(bounce, stores[0] + from, payload, cudaMemcpyDeviceToHost, st);
+			if (ok && payload) e = cudaMemcpyAsync(bounce, reps[0].store + from, payload, cudaMemcpyDeviceToHost, st);
 			break;
 		case 1:		/* NBD_CMD_WRITE */
 			ok = range_ok;
-			for (int r = 0; ok && payload && r < nrep && e == cudaSuccess; r++)
-				e = cudaMemcpyAsync(stores[r] + from, bounce, payload, cudaMemcpyHostToDevice, st);
+			for (size_t r = 0; ok && payload && r < reps.size() && e == cudaSuccess; r++)
+				e = cudaMemcpyAsync(reps[r].store + from, bounce, payload, cudaMemcpyHostToDevice, st);
 			break;
 		case 3:		/* NBD_CMD_FLUSH: the whole device, a no-op for RAM */
 			ok = true;
 			break;
 		case 4:		/* NBD_CMD_TRIM -> spdk_bdev_unmap: zero fill; "Can't unmap 0 bytes" (bdev.c:2796-2799) */
 			ok = range_ok && len != 0;
-			for (int r = 0; ok && len && r < nrep && e == cudaSuccess; r++) e = cudaMemsetAsync(stores[r] + from, 0, len, st);
+			for (size_t r = 0; ok && len && r < reps.size() && e == cudaSuccess; r++) e = cudaMemsetAsync(reps[r].store + from, 0, len, st);
 			break;
 		default:	/* unknown command: EIO (nbd.c:527-540) */
 			break;
@@ -128,8 +124,8 @@ extern "C" int oimgpu_nbd_serve(const char *bdev_name, int sock_fd)
 			ParkedPollers parked(-1);
 			cudaFreeHost(bounce);
 		}
+		close_bdev_locked(name);
 		Bdev *b = find_bdev_locked(name.c_str());
-		if (b && b->open_luns > 0) b->open_luns--;
 		if (b && b->nbd_exports > 0) b->nbd_exports--;
 	}
 	if (st) cudaStreamDestroy(st);

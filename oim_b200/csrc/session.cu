@@ -27,8 +27,8 @@ static cudaError_t h2d_sync(oimgpu_lun *L, void *dst, const void *src, size_t n)
  * (vhost_scsi.c:1004-1013); the device id is the slot add_vhost_scsi_lun took in the global table */
 static void fill_lun_ctx(LunCtx &c, const Bdev &b, const Ctrlr &ctrlr, int target)
 {
-	for (size_t r = 0; r < b.stores.size(); r++) c.store[r] = b.stores[r];
-	c.nreplicas = (uint32_t)b.stores.size();
+	for (size_t r = 0; r < b.replicas.size(); r++) c.store[r] = b.replicas[r].store;
+	c.nreplicas = (uint32_t)b.replicas.size();
 	c.num_blocks = b.num_blocks;
 	c.block_size = b.block_size;
 	c.hist = b.hist;
@@ -58,10 +58,10 @@ bool oimgpu::read_ctx_stats(int device, const LunCtx *d_ctx, unsigned long long 
 /* a session lets go of a bdev: keep what it counted (get_bdevs_iostat is per bdev, for its lifetime) */
 static void retire_stats_locked(const std::string &bdev, int device, const LunCtx *d_ctx)
 {
-	auto bi = g.bdevs.find(bdev);
+	Bdev *b = find_bdev_locked(bdev.c_str());
 	unsigned long long v[12];
-	if (bi == g.bdevs.end() || !read_ctx_stats(device, d_ctx, v)) return;
-	for (int k = 0; k < 12; k++) bi->second->retired[k] += v[k];
+	if (!b || !read_ctx_stats(device, d_ctx, v)) return;
+	for (int k = 0; k < 12; k++) b->retired[k] += v[k];
 }
 
 /* Bring the session's view of its controller up to date: every target other than the session's
@@ -78,12 +78,11 @@ static int refresh_peers_locked(oimgpu_lun *L)
 	for (int t = 0; t < OIMGPU_CTRLR_MAX_DEVS; t++) {
 		std::string &want = wants[t];
 		if (it != g.ctrlrs.end() && t != L->target) want = it->second->targets[t];
-		if (!want.empty()) {
-			auto bi = g.bdevs.find(want);
-			if (bi == g.bdevs.end() || !device_reachable(L->device, bi->second->devices[0])) want.clear();
-		}
+		const Bdev *b = want.empty() ? nullptr : find_bdev_locked(want.c_str());
+		if (b && !device_reachable(L->device, b->replicas[0].device)) b = nullptr;
+		if (!b) want.clear();
 		if (want != L->peer_bdev[t] && !L->peer_bdev[t].empty()) restart = true;	/* a device goes away */
-		if (!want.empty() && g.bdevs[want]->stores.size() > 1 && !L->any_mirror) restart = true;	/* other kernel variant */
+		if (b && b->replicas.size() > 1 && !L->any_mirror) restart = true;	/* other kernel variant */
 	}
 	/* a resident poller may be in the middle of a pass on a device that is being unplugged: park it,
 	 * like the reference waits for the session's outstanding tasks (process_removed_devs,
@@ -97,9 +96,10 @@ static int refresh_peers_locked(oimgpu_lun *L)
 		const std::string &want = wants[t];
 		if (want == L->peer_bdev[t]) continue;
 		changed = true;
+		/* before anything changes: a peer target that is named has its context (for_each_ctx visits it) */
+		if (!want.empty() && !L->d_peer[t]) CU_OK(cudaMalloc((void **)&L->d_peer[t], sizeof(LunCtx)));
 		if (!L->peer_bdev[t].empty()) {
-			Bdev *b = find_bdev_locked(L->peer_bdev[t].c_str());
-			if (b && b->open_luns > 0) b->open_luns--;
+			close_bdev_locked(L->peer_bdev[t]);
 			if (!L->poller_active) cudaStreamSynchronize(L->stream);
 			retire_stats_locked(L->peer_bdev[t], L->device, L->d_peer[t]);
 		}
@@ -108,12 +108,11 @@ static int refresh_peers_locked(oimgpu_lun *L)
 			L->h_ctx.peer[t] = nullptr;	/* the context itself is freed at close: a resident kernel may still hold it */
 			continue;
 		}
-		Bdev &b = *g.bdevs[want];
-		b.open_luns++;
+		Bdev &b = *find_bdev_locked(want.c_str());
+		open_bdev_locked(b);
 		LunCtx c;
 		memset(&c, 0, sizeof(c));
 		fill_lun_ctx(c, b, *it->second, t);
-		if (!L->d_peer[t]) CU_OK(cudaMalloc((void **)&L->d_peer[t], sizeof(LunCtx)));
 		CU_OK(cudaMemcpyAsync(L->d_peer[t], &c, sizeof(c), cudaMemcpyHostToDevice, L->copy_stream));
 		CU_OK(cudaStreamSynchronize(L->copy_stream));	/* `c` is pageable stack memory */
 		L->h_ctx.peer[t] = L->d_peer[t];
@@ -124,7 +123,7 @@ static int refresh_peers_locked(oimgpu_lun *L)
 	}
 	L->any_mirror = L->h_ctx.nreplicas > 1;
 	for (int t = 0; t < OIMGPU_CTRLR_MAX_DEVS; t++) {
-		if (!L->peer_bdev[t].empty() && g.bdevs[L->peer_bdev[t]]->stores.size() > 1) L->any_mirror = true;
+		if (!L->peer_bdev[t].empty() && find_bdev_locked(L->peer_bdev[t].c_str())->replicas.size() > 1) L->any_mirror = true;
 	}
 	/* a launch still in flight finishes with the peers it started with: published under it, a mirror attached
 	 * while the plain kernel runs would be served by a kernel that ignores Segment::mirror (GOOD, replica 0 only) */
@@ -148,27 +147,24 @@ void oimgpu::refresh_ctrlr_sessions_locked(const std::string &ctrlr)
 	}
 }
 
-/* Point store[replica] of every device-resident context of bdev `bdev` - a session's own and the peer-target contexts
- * of controller-wide sessions - at `store`.  refresh_peers_locked rebuilds a context only when a target's bdev name
- * changes, so a store that changes under the same name needs this.  Caller holds g.mu and has held and drained every
- * session that reaches the bdev: no kernel reads a context while it changes.  The host copy of a session's own context
- * changes too, since oimgpu_lun_set_removed and oimgpu_lun_set_mem_table upload it whole. */
-int oimgpu::publish_replica_locked(const std::string &bdev, int replica, uint8_t *store)
+/* Write the `len` bytes at `value` at `offset` of every device-resident context of bdev `bdev` - a session's own and
+ * the peer-target contexts of controller-wide sessions.  refresh_peers_locked rebuilds a context only when a target's
+ * bdev name changes, so a field that changes under the same name (a histogram, a replica's store) needs this.  The
+ * caller holds g.mu and makes sure that no kernel reads the field while it changes.  The host copy of a session's own
+ * context changes too, since oimgpu_lun_set_removed and oimgpu_lun_set_mem_table upload it whole. */
+int oimgpu::publish_ctx_locked(const std::string &bdev, size_t offset, const void *value, size_t len)
 {
-	const size_t at = offsetof(LunCtx, store) + sizeof(uint8_t *) * replica;
 	for (oimgpu_lun *L : g.handles) {
 		std::lock_guard<std::recursive_mutex> hl(L->mu);
 		CU_OK(cudaSetDevice(L->device));
-		if (L->bdev == bdev) {
-			L->h_ctx.store[replica] = store;
-			CU_OK(cudaMemcpyAsync((uint8_t *)L->d_ctx + at, &L->h_ctx.store[replica], sizeof(store), cudaMemcpyHostToDevice,
-					      L->copy_stream));
-		}
-		for (int t = 0; t < OIMGPU_CTRLR_MAX_DEVS; t++) {
-			if (L->peer_bdev[t] != bdev || !L->d_peer[t]) continue;
-			CU_OK(cudaMemcpyAsync((uint8_t *)L->d_peer[t] + at, &store, sizeof(store), cudaMemcpyHostToDevice, L->copy_stream));
-		}
-		CU_OK(cudaStreamSynchronize(L->copy_stream));	/* `store` is pageable */
+		int rc = for_each_ctx(L, [&](const std::string &name, LunCtx *d, LunCtx *h) {
+			if (name != bdev) return 0;
+			if (h) memcpy((uint8_t *)h + offset, value, len);
+			CU_OK(cudaMemcpyAsync((uint8_t *)d + offset, value, len, cudaMemcpyHostToDevice, L->copy_stream));
+			return 0;
+		});
+		if (rc) return rc;
+		CU_OK(cudaStreamSynchronize(L->copy_stream));	/* `value` is pageable */
 	}
 	return 0;
 }
@@ -200,10 +196,7 @@ static void free_lun_resources(oimgpu_lun *L)
 	cudaFree(L->d_ctx);
 	for (int t = 0; t < OIMGPU_CTRLR_MAX_DEVS; t++) {
 		cudaFree(L->d_peer[t]);
-		if (!L->peer_bdev[t].empty()) {
-			Bdev *b = find_bdev_locked(L->peer_bdev[t].c_str());
-			if (b && b->open_luns > 0) b->open_luns--;
-		}
+		if (!L->peer_bdev[t].empty()) close_bdev_locked(L->peer_bdev[t]);
 	}
 	if (L->done) cudaEventDestroy(L->done);
 	if (L->stream) cudaStreamDestroy(L->stream);
@@ -227,10 +220,10 @@ static int lun_open_on(const char *ctrlr, int scsi_target_num, int on_device, ui
 		bn = c->targets[scsi_target_num];
 		if (bn.empty()) return -ENODEV;
 	}
-	Bdev *bp = session ? nullptr : g.bdevs[bn].get();
+	Bdev *bp = session ? nullptr : find_bdev_locked(bn.c_str());
 	int session_device = g.devices[0].ordinal;
 	for (int t = 0; session && t < OIMGPU_CTRLR_MAX_DEVS; t++) {
-		if (!c->targets[t].empty()) { session_device = g.bdevs[c->targets[t]]->devices[0]; break; }
+		if (!c->targets[t].empty()) { session_device = find_bdev_locked(c->targets[t].c_str())->replicas[0].device; break; }
 	}
 	if (on_device >= 0) {
 		if (!session || find_device_slot(on_device) < 0) return -EINVAL;
@@ -248,7 +241,7 @@ static int lun_open_on(const char *ctrlr, int scsi_target_num, int on_device, ui
 	L->ctrlr = c->name;
 	L->bdev = bn;
 	L->target = session ? 0xff : scsi_target_num;
-	L->device = session ? session_device : bp->devices[0];
+	L->device = session ? session_device : bp->replicas[0].device;
 	L->sm_count = g.devices[find_device_slot(L->device)].sm_count;
 	L->num_queues = num_queues;
 	L->queue_size = queue_size;
@@ -310,8 +303,7 @@ static int lun_open_on(const char *ctrlr, int scsi_target_num, int on_device, ui
 	L->grid_cap = L->sm_count * per_sm;
 	int rc = refresh_peers_locked(L.get());
 	if (rc) return rc;
-	g.open_luns++;
-	if (bp) bp->open_luns++;
+	if (bp) open_bdev_locked(*bp);
 	g.handles.push_back(L.get());
 	*out = L.release();
 	return 0;
@@ -343,18 +335,16 @@ extern "C" int oimgpu_lun_close(oimgpu_lun *L)
 		L->poller_active = false;
 	}
 	cudaStreamSynchronize(L->stream);
-	if (!L->bdev.empty()) retire_stats_locked(L->bdev, L->device, L->d_ctx);
-	for (int t = 0; t < OIMGPU_CTRLR_MAX_DEVS; t++) {
-		if (!L->peer_bdev[t].empty()) retire_stats_locked(L->peer_bdev[t], L->device, L->d_peer[t]);
-	}
+	for_each_ctx(L, [&](const std::string &bn, LunCtx *d, LunCtx *) {
+		retire_stats_locked(bn, L->device, d);
+		return 0;
+	});
 	{
 		ParkedPollers parked(L->device, L);	/* other sessions' resident kernels */
 		free_lun_resources(L);
 		g.handles.erase(std::remove(g.handles.begin(), g.handles.end(), L), g.handles.end());
 	}
-	g.open_luns--;
-	Bdev *b = find_bdev_locked(L->bdev.c_str());
-	if (b && b->open_luns > 0) b->open_luns--;
+	close_bdev_locked(L->bdev);
 	delete L;
 	return 0;
 }
