@@ -5,8 +5,6 @@
  * The kernel lives here and not in lun_kernel.cu so that nothing it needs can shift the register allocation of
  * the queue kernels; it reuses their unit movers (move_unit, zero_unit in lun_kernel.cuh).
  */
-#include <deque>
-
 #include "host_state.h"
 
 namespace {
@@ -62,9 +60,9 @@ struct oimgpu_bio_chan {
 	 * is built while batch k's upload may still be pending.  (Not a pageable copy: this process may have pinned
 	 * pages next to any heap buffer, and the driver refuses a copy that straddles a registration.) */
 	std::vector<BioSeg> segs;
-	struct Staging { BioSeg *h = nullptr; size_t cap = 0; uint64_t batch = 0; };
+	struct Staging { Buf<BioSeg, Mem::Pinned> h; uint64_t batch = 0; };
 	Staging staging[2];
-	std::vector<BioSeg *> retired_staging;	/* outgrown, freed at close */
+	std::vector<Buf<BioSeg, Mem::Pinned>> retired_staging;	/* outgrown, freed at close: a submit never parks pollers */
 	uint64_t batches = 0, reaped = 0;
 	std::vector<uint32_t> launch_end;	/* segments [launch_end[i-1], launch_end[i]) form launch i */
 	std::vector<uint32_t> launch_units;
@@ -72,9 +70,8 @@ struct oimgpu_bio_chan {
 	size_t d_cap = 0;
 	struct Range { uint64_t lo, hi; bool writes; };
 	std::vector<Range> group;		/* store ranges of the launch being built */
-	struct Batch { cudaEvent_t ev; std::vector<oimgpu_bio_cpl> cpls; size_t next; };
-	std::deque<Batch> inflight;
-	std::vector<cudaEvent_t> spare;
+	struct Batch { std::vector<oimgpu_bio_cpl> cpls; size_t next; };
+	EventFifo<Batch> inflight;
 	unsigned long long launches = 0;
 };
 
@@ -105,18 +102,14 @@ extern "C" int oimgpu_bio_chan_close(oimgpu_bio_chan *c)
 	if (!c) return -EINVAL;
 	cudaSetDevice(c->device);
 	cudaStreamSynchronize(c->stream);
-	for (auto &b : c->inflight) cudaEventDestroy(b.ev);
-	for (auto ev : c->spare) cudaEventDestroy(ev);
 	if (c->d_segs) cudaFreeAsync(c->d_segs, c->stream);	/* stream-ordered: does not wait for the whole device */
 	cudaStreamSynchronize(c->stream);
 	cudaStreamDestroy(c->stream);
 	{
 		std::lock_guard<std::mutex> lk(g.mu);
-		{
-			ParkedPollers parked(c->device);	/* cudaFreeHost waits for the device, like cudaFree */
-			for (auto &st : c->staging) if (st.h) cudaFreeHost(st.h);
-			for (BioSeg *h : c->retired_staging) cudaFreeHost(h);
-		}
+		ParkedPollers parked(kAllGpus);
+		for (auto &st : c->staging) st.h.reset(parked);
+		for (auto &h : c->retired_staging) h.reset(parked);
 		close_bdev_locked(c->bdev);
 	}
 	delete c;
@@ -164,7 +157,7 @@ extern "C" int oimgpu_bio_chan_submit(oimgpu_bio_chan *c, const oimgpu_bio *bios
 {
 	if (!c || (!bios && n) || (!iovs && niovs)) return -EINVAL;
 	if (n == 0) return 0;
-	oimgpu_bio_chan::Batch batch{nullptr, std::vector<oimgpu_bio_cpl>(n), 0};
+	oimgpu_bio_chan::Batch batch{std::vector<oimgpu_bio_cpl>(n), 0};
 	c->segs.clear();
 	c->launch_end.clear();
 	c->launch_units.clear();
@@ -214,18 +207,14 @@ extern "C" int oimgpu_bio_chan_submit(oimgpu_bio_chan *c, const oimgpu_bio *bios
 			c->d_cap = cap;
 		}
 		auto &st = c->staging[seq & 1];
-		if (st.batch > c->reaped) CU_OK(cudaEventSynchronize(c->inflight[st.batch - c->reaped - 1].ev));	/* its upload is queued */
-		if (c->segs.size() > st.cap) {
-			if (st.h) c->retired_staging.push_back(st.h);
-			st.h = nullptr;
-			st.cap = 0;
-			const size_t cap = std::max<size_t>(c->segs.size() * 2, 1024);
-			CU_OK(cudaHostAlloc((void **)&st.h, cap * sizeof(BioSeg), cudaHostAllocDefault));
-			st.cap = cap;
+		if (st.batch > c->reaped) CU_OK(cudaEventSynchronize(c->inflight.entries[st.batch - c->reaped - 1].ev));	/* its upload is queued */
+		if (c->segs.size() > st.h.size()) {
+			if (st.h) c->retired_staging.push_back(std::move(st.h));
+			CU_OK(st.h.alloc(c->device, std::max<size_t>(c->segs.size() * 2, 1024)));
 		}
-		memcpy(st.h, c->segs.data(), bytes);
+		memcpy(st.h.get(), c->segs.data(), bytes);
 		st.batch = seq;
-		CU_OK(cudaMemcpyAsync(c->d_segs, st.h, bytes, cudaMemcpyHostToDevice, c->stream));
+		CU_OK(cudaMemcpyAsync(c->d_segs, st.h.get(), bytes, cudaMemcpyHostToDevice, c->stream));
 		uint32_t s0 = 0;
 		for (size_t l = 0; l < c->launch_end.size(); l++) {
 			const uint32_t s1 = c->launch_end[l], nu = c->launch_units[l];
@@ -236,32 +225,18 @@ extern "C" int oimgpu_bio_chan_submit(oimgpu_bio_chan *c, const oimgpu_bio *bios
 			s0 = s1;
 		}
 	}
-	if (!c->spare.empty()) { batch.ev = c->spare.back(); c->spare.pop_back(); }
-	else CU_OK(cudaEventCreateWithFlags(&batch.ev, cudaEventDisableTiming));
-	CU_OK(cudaEventRecord(batch.ev, c->stream));
-	c->inflight.push_back(std::move(batch));
-	return 0;
+	return c->inflight.record(c->stream, std::move(batch));
 }
 
 extern "C" int oimgpu_bio_chan_poll(oimgpu_bio_chan *c, oimgpu_bio_cpl *out, int max)
 {
 	if (!c || (!out && max > 0)) return -EINVAL;
-	int n = 0;
-	while (n < max && !c->inflight.empty()) {
-		auto &b = c->inflight.front();
-		if (b.next == 0) {
-			cudaError_t e = cudaEventQuery(b.ev);
-			if (e == cudaErrorNotReady) { (void)cudaGetLastError(); break; }
-			if (e != cudaSuccess) { (void)cudaGetLastError(); return -EIO; }
-		}
+	return c->inflight.poll(max, [&](oimgpu_bio_chan::Batch &b, int &n) {
 		while (n < max && b.next < b.cpls.size()) out[n++] = b.cpls[b.next++];
-		if (b.next == b.cpls.size()) {
-			c->spare.push_back(b.ev);
-			c->inflight.pop_front();
-			c->reaped++;
-		}
-	}
-	return n;
+		if (b.next < b.cpls.size()) return false;
+		c->reaped++;
+		return true;
+	});
 }
 
 extern "C" unsigned long long oimgpu_bio_chan_launches(const oimgpu_bio_chan *c) { return c ? c->launches : 0; }

@@ -78,7 +78,7 @@ static void release_store(const Replica &r)
 
 /* Take a bdev apart once nothing uses it: own stores are freed (their bytes given back to their GPU's count, which
  * places later bdevs), imported ones closed, the histogram freed and the name unregistered.  The pollers of each
- * replica's GPU are parked around its release. */
+ * replica's GPU are parked around its release; the histogram goes with replica 0, on whose GPU it lives. */
 static void drop_bdev_locked(Bdev *b)
 {
 	if (!g.control_only) {
@@ -86,10 +86,10 @@ static void drop_bdev_locked(Bdev *b)
 			{
 				ParkedPollers parked(r.device);
 				release_store(r);
+				b->hist.reset(parked);
 			}
 			if (!r.imported) g.devices[find_device_slot(r.device)].bytes_allocated -= b->num_blocks * (uint64_t)b->block_size;
 		}
-		if (b->hist) { cudaSetDevice(b->replicas[0].device); cudaFree(b->hist); }
 	}
 	g.bdev_order.erase(std::remove(g.bdev_order.begin(), g.bdev_order.end(), b->name), g.bdev_order.end());
 	g.bdevs.erase(g.bdevs.find(b->name));
@@ -476,13 +476,13 @@ static int digest_locked(int device, const void *dptr, uint64_t nbytes, uint64_t
 	CU_OK(cudaSetDevice(device));
 	cudaStream_t st = g.devices[slot].util;
 	unsigned long long *d = nullptr;
-	CU_OK(cudaMalloc((void **)&d, 16));
+	CU_OK(cudaMallocAsync((void **)&d, 16, st));	/* stream-ordered: the free does not wait for a resident poller */
 	CU_OK(cudaMemsetAsync(d, 0, 16, st));
 	oim_digest_kernel<<<g.devices[slot].sm_count * 4, 256, 0, st>>>((const uint64_t *)dptr, nbytes / 8, d);
 	unsigned long long h[2] = {0, 0};
 	cudaError_t e = cudaMemcpyAsync(h, d, 16, cudaMemcpyDeviceToHost, st);
 	if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-	cudaFree(d);
+	cudaFreeAsync(d, st);
 	if (e != cudaSuccess) { (void)cudaGetLastError(); return -EIO; }
 	out[0] = h[0]; out[1] = h[1];
 	return 0;
@@ -548,34 +548,25 @@ extern "C" int oimgpu_bdev_histogram_enable(const char *name, int enable)
 	if (!g.inited) return -ENODEV;
 	Bdev *b = find_bdev_locked(name);
 	if (!b) return -ENODEV;
-	if (g.control_only) { b->hist = enable ? (unsigned long long *)1 : nullptr; return 0; }
+	if (g.control_only) return 0;	/* no data path: the histogram reads as empty either way */
 	const int dev0 = b->replicas[0].device;
 	CU_OK(cudaSetDevice(dev0));
 	cudaStream_t st = g.devices[find_device_slot(dev0)].util;
 	/* every open session's device-resident view of the bdev learns where its histogram is (or that it is gone) */
 	if (enable) {
-		if (!b->hist) {
-			unsigned long long *h = nullptr;
-			CU_OK(cudaMalloc((void **)&h, sizeof(unsigned long long) * kHistBuckets));
-			b->hist = h;
-		}
-		CU_OK(cudaMemsetAsync(b->hist, 0, sizeof(unsigned long long) * kHistBuckets, st));
+		if (!b->hist) CU_OK(b->hist.alloc(dev0, kHistBuckets));
+		CU_OK(cudaMemsetAsync(b->hist.get(), 0, sizeof(unsigned long long) * kHistBuckets, st));
 		CU_OK(cudaStreamSynchronize(st));
-		return publish_ctx_locked(b->name, offsetof(LunCtx, hist), &b->hist, sizeof(b->hist));
+	} else if (!b->hist) {
+		return 0;
 	}
-	if (b->hist) {
-		unsigned long long *none = nullptr;
-		int rc = publish_ctx_locked(b->name, offsetof(LunCtx, hist), &none, sizeof(none));
-		if (rc) return rc;
-		/* kernels already launched may still tally: everything in flight first, resident pollers parked */
-		{
-			ParkedPollers parked(-1);
-			(void)sync_session_streams_locked();
-			cudaSetDevice(dev0);
-			cudaFree(b->hist);
-		}
-		b->hist = nullptr;
-	}
+	unsigned long long *h = enable ? b->hist.get() : nullptr;
+	int rc = publish_ctx_locked(b->name, offsetof(LunCtx, hist), &h, sizeof(h));
+	if (rc || enable) return rc;
+	/* kernels already launched may still tally: everything in flight first, resident pollers parked */
+	ParkedPollers parked(kAllGpus);
+	(void)sync_session_streams_locked();
+	b->hist.reset(parked);
 	return 0;
 }
 
@@ -593,7 +584,7 @@ extern "C" int oimgpu_bdev_histogram_get(const char *name, uint64_t *buckets)
 	if (g.control_only) return 0;
 	CU_OK(cudaSetDevice(b->replicas[0].device));
 	cudaStream_t st = g.devices[find_device_slot(b->replicas[0].device)].util;
-	CU_OK(cudaMemcpyAsync(buckets, b->hist, sizeof(uint64_t) * kHistBuckets, cudaMemcpyDeviceToHost, st));
+	CU_OK(cudaMemcpyAsync(buckets, b->hist.get(), sizeof(uint64_t) * kHistBuckets, cudaMemcpyDeviceToHost, st));
 	CU_OK(cudaStreamSynchronize(st));
 	return 0;
 }

@@ -1,8 +1,6 @@
 /*
  * copy_chan.cu - host memory for the GPU (registration, on-demand pinning) and the asynchronous copy channel.
  */
-#include <deque>
-
 #include "host_state.h"
 
 extern "C" int oimgpu_mem_register(void *addr, size_t len)
@@ -44,7 +42,7 @@ extern "C" int oimgpu_mem_unregister(void *addr)
 	 * needs: with a resident poller anywhere that is a deadlock, not a delay (seen: one VM's teardown
 	 * against another VM's poller restart).  Same remedy as for cudaFree. */
 	{
-		ParkedPollers parked(-1);
+		ParkedPollers parked(kAllGpus);
 		cudaHostUnregister(addr);
 	}
 	g.registered.erase(it);
@@ -169,10 +167,7 @@ struct oimgpu_copy_chan {
 	int device = 0;
 	int sm_count = 0;
 	cudaStream_t stream = nullptr;
-	struct Op { cudaEvent_t ev; void *tag; };
-	std::deque<Op> inflight;
-	std::vector<cudaEvent_t> spare;
-	unsigned long long launches = 0;
+	EventFifo<void *> inflight;	/* the tag of each copy or fill */
 };
 
 extern "C" int oimgpu_copy_chan_open(int device, oimgpu_copy_chan **out)
@@ -197,21 +192,8 @@ extern "C" int oimgpu_copy_chan_close(oimgpu_copy_chan *c)
 	if (!c) return -EINVAL;
 	cudaSetDevice(c->device);
 	cudaStreamSynchronize(c->stream);
-	for (auto &op : c->inflight) cudaEventDestroy(op.ev);
-	for (auto ev : c->spare) cudaEventDestroy(ev);
 	cudaStreamDestroy(c->stream);
 	delete c;
-	return 0;
-}
-
-static int chan_record(oimgpu_copy_chan *c, void *tag)
-{
-	cudaEvent_t ev;
-	if (!c->spare.empty()) { ev = c->spare.back(); c->spare.pop_back(); }
-	else CU_OK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-	CU_OK(cudaEventRecord(ev, c->stream));
-	c->inflight.push_back({ev, tag});
-	c->launches++;
 	return 0;
 }
 
@@ -223,7 +205,7 @@ extern "C" int oimgpu_copy_chan_copy(oimgpu_copy_chan *c, void *dst, const void 
 	if (rc) return rc;
 	CU_OK(cudaSetDevice(c->device));
 	if (nbytes) CU_OK(launch_copy(c->stream, c->sm_count, dst, src, nbytes));
-	return chan_record(c, tag);
+	return c->inflight.record(c->stream, tag);
 }
 
 extern "C" int oimgpu_copy_chan_fill(oimgpu_copy_chan *c, void *dst, uint8_t fill, uint64_t nbytes, void *tag)
@@ -233,22 +215,13 @@ extern "C" int oimgpu_copy_chan_fill(oimgpu_copy_chan *c, void *dst, uint8_t fil
 	if (rc) return rc;
 	CU_OK(cudaSetDevice(c->device));
 	if (nbytes) CU_OK(launch_fill(c->stream, c->sm_count, dst, fill, nbytes));
-	return chan_record(c, tag);
+	return c->inflight.record(c->stream, tag);
 }
 
 extern "C" int oimgpu_copy_chan_poll(oimgpu_copy_chan *c, void **tags, int max)
 {
 	if (!c || (!tags && max > 0)) return -EINVAL;
-	int n = 0;
-	while (n < max && !c->inflight.empty()) {
-		cudaError_t e = cudaEventQuery(c->inflight.front().ev);
-		if (e == cudaErrorNotReady) { (void)cudaGetLastError(); break; }
-		if (e != cudaSuccess) { (void)cudaGetLastError(); return -EIO; }
-		tags[n++] = c->inflight.front().tag;
-		c->spare.push_back(c->inflight.front().ev);
-		c->inflight.pop_front();
-	}
-	return n;
+	return c->inflight.poll(max, [&](void *tag, int &n) { tags[n++] = tag; return true; });
 }
 
-extern "C" unsigned long long oimgpu_copy_chan_launches(const oimgpu_copy_chan *c) { return c ? c->launches : 0; }
+extern "C" unsigned long long oimgpu_copy_chan_launches(const oimgpu_copy_chan *c) { return c ? c->inflight.recorded : 0; }

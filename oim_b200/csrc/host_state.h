@@ -1,7 +1,7 @@
 /*
  * host_state.h - what the host-side files of liboimgpu.so (control.cu, session.cu, nbd.cu, copy_chan.cu, bio_chan.cu,
- * mirror_check.cu) share:
- * the registry, the session, and the helpers more than one of them calls.  Internal, not installed.
+ * mirror_check.cu) share: the registry, the session, the helpers more than one of them calls, the Buf that owns device and
+ * pinned memory and frees it only under a ParkedPollers scope, and the channels' EventFifo.  Internal, not installed.
  */
 #pragma once
 
@@ -13,6 +13,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <deque>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -32,6 +33,97 @@
 	} while (0)
 
 namespace oimgpu {
+
+struct ParkedPollers;
+constexpr int kAllGpus = -1, kNoGpu = -2;	/* ParkedPollers devices besides one GPU's ordinal */
+
+/* Device memory (cudaMalloc) or pinned host memory (cudaHostAlloc, plain or mapped) of the library: pointer, element count
+ * and GPU.  Freeing it waits for that GPU (pinned: every GPU), so it is freed only under a ParkedPollers scope that covers
+ * them, which release() checks.  A failed allocation leaves it empty.  It never frees itself: memory still held when it
+ * is destroyed stays with the process (the registry's, at exit without oimgpu_fini). */
+enum class Mem { Device, Pinned, Mapped };
+
+template <class T, Mem K> class Buf {
+public:
+	Buf() = default;
+	Buf(Buf &&o) noexcept : p_(o.p_), n_(o.n_), device_(o.device_) { o.p_ = nullptr; o.n_ = 0; }
+	T *get() const { return p_; }
+	T &operator[](size_t i) const { return p_[i]; }
+	explicit operator bool() const { return p_ != nullptr; }
+	size_t size() const { return n_; }
+	/* the GPUs whose pollers a free waits for, as a ParkedPollers device */
+	int waits_for() const { return !p_ ? kNoGpu : K == Mem::Device ? device_ : kAllGpus; }
+	/* n elements on GPU `device`, into an empty buffer (a live one would have to be freed without a scope) */
+	cudaError_t alloc(int device, size_t n)
+	{
+		release(nullptr);
+		cudaError_t e = cudaSetDevice(device);
+		if (e == cudaSuccess) e = K == Mem::Device ? cudaMalloc((void **)&p_, n * sizeof(T))
+							   : cudaHostAlloc((void **)&p_, n * sizeof(T), K == Mem::Mapped ? cudaHostAllocMapped : cudaHostAllocDefault);
+		if (e != cudaSuccess) {
+			(void)cudaGetLastError();	/* a refusal must not surface at a later launch check */
+			p_ = nullptr;
+			return e;
+		}
+		n_ = n;
+		device_ = device;
+		return e;
+	}
+	/* at least n elements: a smaller buffer is freed under `parked` and replaced (contents are not kept) */
+	cudaError_t grow(int device, size_t n, const ParkedPollers &parked)
+	{
+		if (n <= n_) return cudaSuccess;
+		release(&parked);
+		return alloc(device, n);
+	}
+	void reset(const ParkedPollers &parked) { release(&parked); }
+private:
+	void release(const ParkedPollers *parked);
+	T *p_ = nullptr;
+	size_t n_ = 0;
+	int device_ = -1;
+};
+
+/* A channel's work in stream order: each piece's payload (a tag, a batch of completions) and the event recorded behind it.
+ * Finished entries leave at the front; events are reused, and destroyed with the FIFO once the stream has drained. */
+template <class P> struct EventFifo {
+	struct Entry { cudaEvent_t ev; P payload; };
+	std::deque<Entry> entries;
+	std::vector<cudaEvent_t> spare;
+	unsigned long long recorded = 0;
+	EventFifo() = default;
+	EventFifo(const EventFifo &) = delete;
+	~EventFifo()
+	{
+		for (auto &e : entries) cudaEventDestroy(e.ev);
+		for (auto ev : spare) cudaEventDestroy(ev);
+	}
+	int record(cudaStream_t st, P payload)
+	{
+		cudaEvent_t ev;
+		if (!spare.empty()) { ev = spare.back(); spare.pop_back(); }
+		else CU_OK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+		CU_OK(cudaEventRecord(ev, st));
+		entries.push_back({ev, std::move(payload)});
+		recorded++;
+		return 0;
+	}
+	/* Up to max results from finished entries, oldest first: take(payload, n) adds its results at n, and returns
+	 * false to keep an entry it could not finish.  The count, or -EIO when an entry's work failed. */
+	template <class Take> int poll(int max, Take take)
+	{
+		int n = 0;
+		while (n < max && !entries.empty()) {
+			const cudaError_t e = cudaEventQuery(entries.front().ev);
+			if (e == cudaErrorNotReady) { (void)cudaGetLastError(); break; }
+			if (e != cudaSuccess) { (void)cudaGetLastError(); return -EIO; }
+			if (!take(entries.front().payload, n)) break;
+			spare.push_back(entries.front().ev);
+			entries.pop_front();
+		}
+		return n;
+	}
+};
 
 struct Device {
 	int ordinal = -1;
@@ -57,7 +149,7 @@ struct Bdev {
 	int opens = 0;		/* open_bdev_locked: session targets (own and peer), NBD exports, bio channels */
 	int nbd_exports = 0;	/* oimgpu_nbd_serve calls serving it (also counted in opens) */
 	std::vector<Replica> replicas;
-	unsigned long long *hist = nullptr;	/* enable_bdev_histogram: kHistBuckets counters on replica 0's GPU */
+	Buf<unsigned long long, Mem::Device> hist;	/* enable_bdev_histogram: kHistBuckets counters on replica 0's GPU */
 	unsigned long long retired[12] = {};	/* counters of sessions that are gone (same layout as LunCtx::stats) */
 };
 
@@ -153,20 +245,20 @@ struct oimgpu_lun {
 	int sm_count = 0;
 	cudaStream_t stream = nullptr;
 	cudaEvent_t done = nullptr;
-	LunCtx *d_ctx = nullptr;
+	Buf<LunCtx, Mem::Device> d_ctx;
 	LunCtx h_ctx{};
 	uint32_t num_queues = 0, queue_size = 0, iov_cap = 0;
 	std::vector<Queue> queues;
 	/* pinned staging ring for {KickHeader, QueueDesc[]}: a slot is reused only after its upload ran */
 	static constexpr int kKickSlots = 4;
-	uint8_t *h_kick[kKickSlots] = {};
+	Buf<uint8_t, Mem::Pinned> h_kick[kKickSlots];
 	cudaEvent_t kick_ev[kKickSlots] = {};
 	uint64_t kicks = 0;
-	uint8_t *d_kick = nullptr;
+	Buf<uint8_t, Mem::Device> d_kick;
 	QueueDesc *d_desc = nullptr;
-	QShare *d_share = nullptr;		/* [3 x num_queues] coordination blocks of shared queues (lun_kernel.cuh) */
+	Buf<QShare, Mem::Device> d_share;	/* [3 x num_queues] coordination blocks of shared queues (lun_kernel.cuh) */
 	/* the session's recent read / write mix: LunCtx::mix, copied here (pinned) behind every launch */
-	volatile unsigned long long *h_mix = nullptr;
+	Buf<volatile unsigned long long, Mem::Pinned> h_mix;
 	unsigned long long mix_seen[2] = {0, 0};
 	bool write_hot = false;
 	uint64_t shared_launches = 0;
@@ -175,30 +267,30 @@ struct oimgpu_lun {
 	/* staged batch path (oimgpu_submit_batch with host arrays): metadata is uploaded by the copy
 	 * engine and the kernel runs on HBM-resident request/SG/completion arrays, so only payload is
 	 * touched over PCIe by the SMs (tools/e2e_probe.py compares the two) */
-	oimgpu_req *bs_d_reqs = nullptr;
-	oimgpu_iov *bs_d_iovs = nullptr;
-	oimgpu_cpl *bs_d_cpls = nullptr;
-	uint8_t *bs_h_pin = nullptr;		/* pinned bounce buffer for pageable caller arrays */
-	size_t bs_cap_reqs = 0, bs_cap_iovs = 0, bs_h_cap = 0;
+	Buf<oimgpu_req, Mem::Device> bs_d_reqs;
+	Buf<oimgpu_iov, Mem::Device> bs_d_iovs;
+	Buf<oimgpu_cpl, Mem::Device> bs_d_cpls;
+	Buf<uint8_t, Mem::Pinned> bs_h_pin;	/* bounce buffer for pageable caller arrays */
 	oimgpu_cpl *bs_user_cpls = nullptr;	/* pending copy-out at wait time */
 	const oimgpu_cpl *bs_h_cpls = nullptr;
 	size_t bs_pending = 0;
 	cudaStream_t copy_stream = nullptr;
 	/* persistent poller */
 	struct Door { volatile uint32_t tail; uint32_t pad0[15]; volatile uint32_t done; uint32_t pad1[15]; };
-	Door *h_door = nullptr, *d_door = nullptr;	/* mapped pinned: one doorbell/completion-count pair per queue */
-	volatile uint32_t *h_flags = nullptr;	/* mapped pinned: [0] stop, [16] exited */
+	Buf<Door, Mem::Mapped> h_door;		/* one doorbell/completion-count pair per queue */
+	Door *d_door = nullptr;
+	Buf<volatile uint32_t, Mem::Mapped> h_flags;	/* [0] stop, [16] exited */
 	uint32_t *d_flags = nullptr;
 	bool poller_active = false;
 	uint32_t poller_grid = 0;
 	uint32_t poller_max_ctas = 0, poller_idle_ms = 0;	/* as given to start_poller: reused when a hot-unplug restarts it */
 	/* the other SCSI devices of the controller, reachable through the same queues (LunCtx::peer) */
-	LunCtx *d_peer[OIMGPU_CTRLR_MAX_DEVS] = {};
+	Buf<LunCtx, Mem::Device> d_peer[OIMGPU_CTRLR_MAX_DEVS];
 	std::string peer_bdev[OIMGPU_CTRLR_MAX_DEVS];
 	bool any_mirror = false;
-	VqState *d_vq_state = nullptr;		/* [num_queues] ring cursors */
-	oimgpu_iov *d_iov_scratch = nullptr;	/* [grid_cap][32][kIovRow] SG rows built by the parser lanes */
-	uint8_t *slab = nullptr;		/* the mapped pinned slab the per-queue rings are carved from */
+	Buf<VqState, Mem::Device> d_vq_state;	/* [num_queues] ring cursors */
+	Buf<oimgpu_iov, Mem::Device> d_iov_scratch;	/* [grid_cap][32][kIovRow] SG rows built by the parser lanes */
+	Buf<uint8_t, Mem::Mapped> slab;	/* the slab the per-queue rings are carved from */
 };
 
 /* Visit the device-resident LunCtxs of session L with the name of the bdev each serves: its own context (passed with
@@ -207,28 +299,30 @@ struct oimgpu_lun {
 template <class Visit> int for_each_ctx(oimgpu_lun *L, Visit visit)
 {
 	if (!L->bdev.empty()) {
-		if (int rc = visit(L->bdev, L->d_ctx, &L->h_ctx)) return rc;
+		if (int rc = visit(L->bdev, L->d_ctx.get(), &L->h_ctx)) return rc;
 	}
 	for (int t = 0; t < OIMGPU_CTRLR_MAX_DEVS; t++) {
 		if (L->peer_bdev[t].empty()) continue;
-		if (int rc = visit(L->peer_bdev[t], L->d_peer[t], (LunCtx *)nullptr)) return rc;
+		if (int rc = visit(L->peer_bdev[t], L->d_peer[t].get(), (LunCtx *)nullptr)) return rc;
 	}
 	return 0;
 }
 
-/* cudaFree waits for the whole device, and a resident poller kernel never finishes on its own: park
- * the pollers of that GPU around a free and bring them back afterwards.  Every session of the GPU is
+namespace oimgpu {
+
+/* cudaFree, cudaFreeHost and cudaHostUnregister wait for the GPU, and a resident poller kernel never finishes on its
+ * own: park the pollers of that GPU around a free and bring them back afterwards.  Every session of the GPU is
  * held (its mutex taken) for the duration, so that none can start a resident kernel in the window -
  * their owners' calls simply wait.  Caller holds g.mu; sessions never take g.mu while holding their own
  * mutex, so the order g.mu -> session mutex is safe.  The pollers stay parked for the scope's lifetime. */
 struct ParkedPollers {
-	/* device < 0: every GPU (pinned host memory is mapped into all of them) */
-	explicit ParkedPollers(int device, oimgpu_lun *except = nullptr)
+	/* device: one GPU, kAllGpus (pinned host memory is mapped into all of them) or kNoGpu */
+	explicit ParkedPollers(int device, oimgpu_lun *except = nullptr) : gpu(device)
 	{
-		park([&](oimgpu_lun *L) { return L != except && (device < 0 || L->device == device); });
+		park([&](oimgpu_lun *L) { return L != except && (device == kAllGpus || L->device == device); });
 	}
 	/* every session on GPU `device`, and every session that reaches bdev `bdev` (its own target or a peer target) */
-	ParkedPollers(int device, const std::string &bdev)
+	ParkedPollers(int device, const std::string &bdev) : gpu(device)
 	{
 		park([&](oimgpu_lun *L) {
 			return L->device == device ||
@@ -256,6 +350,7 @@ struct ParkedPollers {
 
 	struct Session { oimgpu_lun *L; bool restart; };
 	std::vector<Session> parked;
+	const int gpu;	/* as constructed: a Buf checks it before it frees */
 
 private:
 	template <class Want> void park(Want want)
@@ -270,3 +365,19 @@ private:
 	}
 };
 
+template <class T, Mem K> void Buf<T, K>::release(const ParkedPollers *parked)
+{
+	if (!p_) return;
+	if (!parked || (parked->gpu != kAllGpus && parked->gpu != waits_for())) {
+		fprintf(stderr, "oimgpu: internal error: memory freed outside a ParkedPollers scope that covers its GPUs\n");
+		abort();
+	}
+	cudaSetDevice(device_);
+	if (K == Mem::Device) cudaFree((void *)p_);
+	else cudaFreeHost((void *)p_);
+	(void)cudaGetLastError();
+	p_ = nullptr;
+	n_ = 0;
+}
+
+}  // namespace oimgpu

@@ -55,8 +55,7 @@ extern "C" int oimgpu_nbd_serve(const char *bdev_name, int sock_fd)
 	}
 	int rc = 0;
 	cudaStream_t st = nullptr;
-	uint8_t *bounce = nullptr;
-	size_t cap = 0;
+	Buf<uint8_t, Mem::Pinned> bounce;
 	cudaSetDevice(reps[0].device);
 	if (cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking) != cudaSuccess) rc = -EIO;
 	auto book = [&](int op, uint64_t bytes) {	/* get_bdevs_iostat counts these like any other bdev I/O */
@@ -75,16 +74,12 @@ extern "C" int oimgpu_nbd_serve(const char *bdev_name, int sock_fd)
 		uint64_t from = 0;
 		for (int k = 0; k < 8; k++) from = from << 8 | req[16 + k];
 		const uint32_t payload = (type == 0 || type == 1) ? len : 0;	/* only READ / WRITE carry one */
-		if (payload > cap) {
-			if (bounce) {
-				std::lock_guard<std::mutex> lk(g.mu);
-				ParkedPollers parked(-1);
-				cudaFreeHost(bounce);
-			}
-			cap = ((size_t)payload + (1u << 20) - 1) & ~(size_t)((1u << 20) - 1);
-			if (cudaHostAlloc((void **)&bounce, cap, cudaHostAllocDefault) != cudaSuccess) { bounce = nullptr; cap = 0; rc = -ENOMEM; break; }
+		if (payload > bounce.size()) {
+			std::lock_guard<std::mutex> lk(g.mu);
+			const size_t cap = ((size_t)payload + (1u << 20) - 1) & ~(size_t)((1u << 20) - 1);
+			if (bounce.grow(reps[0].device, cap, ParkedPollers(bounce.waits_for())) != cudaSuccess) { rc = -ENOMEM; break; }
 		}
-		if (type == 1 && payload && !read_full(sock_fd, bounce, payload)) break;
+		if (type == 1 && payload && !read_full(sock_fd, bounce.get(), payload)) break;
 		if (type == 2) break;	/* NBD_CMD_DISC: nothing outstanding here, close */
 		/* spdk_bdev_bytes_to_blocks + spdk_bdev_io_valid_blocks (bdev.c:2474-2509): whole blocks, inside the device */
 		const bool range_ok = from % bs == 0 && len % bs == 0 && from <= size && len <= size - from;
@@ -93,12 +88,12 @@ extern "C" int oimgpu_nbd_serve(const char *bdev_name, int sock_fd)
 		switch (type) {
 		case 0:		/* NBD_CMD_READ */
 			ok = range_ok;
-			if (ok && payload) e = cudaMemcpyAsync(bounce, reps[0].store + from, payload, cudaMemcpyDeviceToHost, st);
+			if (ok && payload) e = cudaMemcpyAsync(bounce.get(), reps[0].store + from, payload, cudaMemcpyDeviceToHost, st);
 			break;
 		case 1:		/* NBD_CMD_WRITE */
 			ok = range_ok;
 			for (size_t r = 0; ok && payload && r < reps.size() && e == cudaSuccess; r++)
-				e = cudaMemcpyAsync(reps[r].store + from, bounce, payload, cudaMemcpyHostToDevice, st);
+				e = cudaMemcpyAsync(reps[r].store + from, bounce.get(), payload, cudaMemcpyHostToDevice, st);
 			break;
 		case 3:		/* NBD_CMD_FLUSH: the whole device, a no-op for RAM */
 			ok = true;
@@ -116,14 +111,11 @@ extern "C" int oimgpu_nbd_serve(const char *bdev_name, int sock_fd)
 		uint8_t resp[16] = {0x67, 0x44, 0x66, 0x98, 0, 0, 0, (uint8_t)(ok ? 0 : EIO)};	/* struct nbd_reply */
 		memcpy(resp + 8, req + 8, 8);
 		if (!write_full(sock_fd, resp, sizeof(resp))) break;
-		if (type == 0 && ok && payload && !write_full(sock_fd, bounce, payload)) break;
+		if (type == 0 && ok && payload && !write_full(sock_fd, bounce.get(), payload)) break;
 	}
 	{
 		std::lock_guard<std::mutex> lk(g.mu);
-		if (bounce) {
-			ParkedPollers parked(-1);
-			cudaFreeHost(bounce);
-		}
+		bounce.reset(ParkedPollers(bounce.waits_for()));
 		close_bdev_locked(name);
 		Bdev *b = find_bdev_locked(name.c_str());
 		if (b && b->nbd_exports > 0) b->nbd_exports--;

@@ -31,7 +31,7 @@ static void fill_lun_ctx(LunCtx &c, const Bdev &b, const Ctrlr &ctrlr, int targe
 	c.nreplicas = (uint32_t)b.replicas.size();
 	c.num_blocks = b.num_blocks;
 	c.block_size = b.block_size;
-	c.hist = b.hist;
+	c.hist = b.hist.get();
 	c.block_shift = (b.block_size & (b.block_size - 1)) ? 0xffffffffu : (uint32_t)__builtin_ctz(b.block_size);
 	c.target = (uint8_t)target;
 	snprintf(c.bdev_name, sizeof(c.bdev_name), "%s", b.name.c_str());
@@ -97,11 +97,11 @@ static int refresh_peers_locked(oimgpu_lun *L)
 		if (want == L->peer_bdev[t]) continue;
 		changed = true;
 		/* before anything changes: a peer target that is named has its context (for_each_ctx visits it) */
-		if (!want.empty() && !L->d_peer[t]) CU_OK(cudaMalloc((void **)&L->d_peer[t], sizeof(LunCtx)));
+		if (!want.empty() && !L->d_peer[t]) CU_OK(L->d_peer[t].alloc(L->device, 1));
 		if (!L->peer_bdev[t].empty()) {
 			close_bdev_locked(L->peer_bdev[t]);
 			if (!L->poller_active) cudaStreamSynchronize(L->stream);
-			retire_stats_locked(L->peer_bdev[t], L->device, L->d_peer[t]);
+			retire_stats_locked(L->peer_bdev[t], L->device, L->d_peer[t].get());
 		}
 		L->peer_bdev[t] = want;
 		if (want.empty()) {
@@ -113,9 +113,9 @@ static int refresh_peers_locked(oimgpu_lun *L)
 		LunCtx c;
 		memset(&c, 0, sizeof(c));
 		fill_lun_ctx(c, b, *it->second, t);
-		CU_OK(cudaMemcpyAsync(L->d_peer[t], &c, sizeof(c), cudaMemcpyHostToDevice, L->copy_stream));
+		CU_OK(cudaMemcpyAsync(L->d_peer[t].get(), &c, sizeof(c), cudaMemcpyHostToDevice, L->copy_stream));
 		CU_OK(cudaStreamSynchronize(L->copy_stream));	/* `c` is pageable stack memory */
-		L->h_ctx.peer[t] = L->d_peer[t];
+		L->h_ctx.peer[t] = L->d_peer[t].get();
 	}
 	if (!changed) {
 		if (restart && was_polling) return oimgpu_lun_start_poller(L, L->poller_max_ctas, L->poller_idle_ms) < 0 ? -EIO : 0;
@@ -130,7 +130,7 @@ static int refresh_peers_locked(oimgpu_lun *L)
 	if (!L->poller_active) CU_OK(cudaStreamSynchronize(L->stream));
 	/* publish the pointers after the contexts they point at (same stream); a separate stream so that a
 	 * resident poller kernel on L->stream does not block the update */
-	CU_OK(cudaMemcpyAsync((uint8_t *)L->d_ctx + offsetof(LunCtx, peer), L->h_ctx.peer, sizeof(L->h_ctx.peer),
+	CU_OK(cudaMemcpyAsync((uint8_t *)L->d_ctx.get() + offsetof(LunCtx, peer), L->h_ctx.peer, sizeof(L->h_ctx.peer),
 			      cudaMemcpyHostToDevice, L->copy_stream));
 	CU_OK(cudaStreamSynchronize(L->copy_stream));
 	if (restart && was_polling) {
@@ -171,36 +171,26 @@ int oimgpu::publish_ctx_locked(const std::string &bdev, size_t offset, const voi
 
 /* ---- data path ----------------------------------------------------------------------------------- */
 
-/* everything a session allocated, whether oimgpu_lun_open got through or not (every member starts null).
- * Caller holds g.mu and has parked the other sessions' pollers (the frees wait for the device). */
-static void free_lun_resources(oimgpu_lun *L)
+/* Take session L apart, whether lun_open_on got through or not (every member starts empty).  Caller holds g.mu and has
+ * stopped L's poller.  L's pinned memory is mapped into every GPU: the other sessions' pollers are parked on all of them. */
+static void destroy_session_locked(oimgpu_lun *L)
 {
+	ParkedPollers parked(kAllGpus, L);
+	auto reset = [&](auto &...buf) { (buf.reset(parked), ...); };
+	reset(L->h_door, L->h_mix, L->h_flags, L->slab, L->bs_h_pin, L->d_kick, L->d_share, L->d_vq_state,
+	      L->d_iov_scratch, L->bs_d_reqs, L->bs_d_iovs, L->bs_d_cpls, L->d_ctx);
+	for (auto &h : L->h_kick) h.reset(parked);
+	for (auto &d : L->d_peer) d.reset(parked);
 	cudaSetDevice(L->device);
-	if (L->h_door) cudaFreeHost((void *)L->h_door);
-	if (L->h_mix) cudaFreeHost((void *)L->h_mix);
-	if (L->h_flags) cudaFreeHost((void *)L->h_flags);
-	if (L->slab) cudaFreeHost(L->slab);
-	for (int k = 0; k < oimgpu_lun::kKickSlots; k++) {
-		if (L->h_kick[k]) cudaFreeHost(L->h_kick[k]);
-		if (L->kick_ev[k]) cudaEventDestroy(L->kick_ev[k]);
-	}
-	cudaFree(L->d_kick);
-	cudaFree(L->d_share);
-	cudaFree(L->d_vq_state);
-	cudaFree(L->d_iov_scratch);
-	cudaFree(L->bs_d_reqs);
-	cudaFree(L->bs_d_iovs);
-	cudaFree(L->bs_d_cpls);
-	if (L->bs_h_pin) cudaFreeHost(L->bs_h_pin);
+	for (cudaEvent_t ev : L->kick_ev) if (ev) cudaEventDestroy(ev);
 	if (L->copy_stream) cudaStreamDestroy(L->copy_stream);
-	cudaFree(L->d_ctx);
-	for (int t = 0; t < OIMGPU_CTRLR_MAX_DEVS; t++) {
-		cudaFree(L->d_peer[t]);
-		if (!L->peer_bdev[t].empty()) close_bdev_locked(L->peer_bdev[t]);
-	}
 	if (L->done) cudaEventDestroy(L->done);
 	if (L->stream) cudaStreamDestroy(L->stream);
 	(void)cudaGetLastError();
+	g.handles.erase(std::remove(g.handles.begin(), g.handles.end(), L), g.handles.end());
+	close_bdev_locked(L->bdev);
+	for (const std::string &p : L->peer_bdev) close_bdev_locked(p);
+	delete L;
 }
 
 static int lun_open_on(const char *ctrlr, int scsi_target_num, int on_device, uint32_t num_queues, uint32_t queue_size, oimgpu_lun **out)
@@ -230,14 +220,8 @@ static int lun_open_on(const char *ctrlr, int scsi_target_num, int on_device, ui
 		session_device = on_device;
 	}
 
-	/* whatever a failed step leaves behind (streams, events, pinned and device allocations) is released here */
-	struct Guard {
-		oimgpu_lun *L;
-		~Guard() { if (L) { free_lun_resources(L); delete L; } }
-		oimgpu_lun *operator->() { return L; }
-		oimgpu_lun *get() { return L; }
-		oimgpu_lun *release() { oimgpu_lun *r = L; L = nullptr; return r; }
-	} L{new oimgpu_lun()};
+	/* whatever a failed step leaves behind (streams, events, buffers, bdev uses) is released here */
+	std::unique_ptr<oimgpu_lun, void (*)(oimgpu_lun *)> L(new oimgpu_lun(), destroy_session_locked);
 	L->ctrlr = c->name;
 	L->bdev = bn;
 	L->target = session ? 0xff : scsi_target_num;
@@ -246,6 +230,7 @@ static int lun_open_on(const char *ctrlr, int scsi_target_num, int on_device, ui
 	L->num_queues = num_queues;
 	L->queue_size = queue_size;
 	L->iov_cap = queue_size * 8 < 1024 ? 1024 : queue_size * 8;	/* power of two >= 7 x 129 */
+	if (bp) open_bdev_locked(*bp);
 	CU_OK(cudaSetDevice(L->device));
 	CU_OK(cudaStreamCreateWithFlags(&L->stream, cudaStreamNonBlocking));
 	CU_OK(cudaStreamCreateWithFlags(&L->copy_stream, cudaStreamNonBlocking));
@@ -254,26 +239,25 @@ static int lun_open_on(const char *ctrlr, int scsi_target_num, int on_device, ui
 	memset(&L->h_ctx, 0, sizeof(L->h_ctx));
 	if (session) L->h_ctx.target = 0xff;
 	else fill_lun_ctx(L->h_ctx, *bp, *c, scsi_target_num);
-	CU_OK(cudaHostAlloc((void **)&L->h_mix, 64, cudaHostAllocDefault));
-	memset((void *)L->h_mix, 0, 64);
+	CU_OK(L->h_mix.alloc(L->device, 8));
+	memset((void *)L->h_mix.get(), 0, 64);
 	L->any_mirror = L->h_ctx.nreplicas > 1;
-	CU_OK(cudaMalloc((void **)&L->d_ctx, sizeof(LunCtx)));
-	CU_OK(h2d_sync(L.get(), L->d_ctx, &L->h_ctx, sizeof(LunCtx)));
+	CU_OK(L->d_ctx.alloc(L->device, 1));
+	CU_OK(h2d_sync(L.get(), L->d_ctx.get(), &L->h_ctx, sizeof(LunCtx)));
 
 	for (int k = 0; k < oimgpu_lun::kKickSlots; k++) {
-		CU_OK(cudaHostAlloc((void **)&L->h_kick[k], sizeof(KickHeader) + sizeof(QueueDesc) * num_queues * 3, cudaHostAllocDefault));
-		memset(L->h_kick[k], 0, sizeof(KickHeader));
+		CU_OK(L->h_kick[k].alloc(L->device, sizeof(KickHeader) + sizeof(QueueDesc) * num_queues * 3));
+		memset(L->h_kick[k].get(), 0, sizeof(KickHeader));
 		CU_OK(cudaEventCreateWithFlags(&L->kick_ev[k], cudaEventDisableTiming));
 	}
-	CU_OK(cudaMalloc((void **)&L->d_kick, sizeof(KickHeader) + sizeof(QueueDesc) * num_queues * 3));	/* ring + device-array + virtqueue per queue */
-	L->d_desc = (QueueDesc *)(L->d_kick + sizeof(KickHeader));
-	CU_OK(cudaMalloc((void **)&L->d_share, sizeof(QShare) * num_queues * 3));
+	CU_OK(L->d_kick.alloc(L->device, sizeof(KickHeader) + sizeof(QueueDesc) * num_queues * 3));	/* ring + device-array + virtqueue per queue */
+	L->d_desc = (QueueDesc *)(L->d_kick.get() + sizeof(KickHeader));
+	CU_OK(L->d_share.alloc(L->device, (size_t)num_queues * 3));
 	L->queues.resize(num_queues);
 	/* one mapped pinned slab per LUN, carved into per-queue rings: the "virtqueues" */
 	const size_t per_q = sizeof(oimgpu_req) * queue_size + sizeof(oimgpu_iov) * L->iov_cap + sizeof(oimgpu_cpl) * queue_size;
-	uint8_t *slab = nullptr, *dslab = nullptr;
-	CU_OK(cudaHostAlloc((void **)&slab, per_q * num_queues, cudaHostAllocMapped));
-	L->slab = slab;
+	CU_OK(L->slab.alloc(L->device, per_q * num_queues));
+	uint8_t *slab = L->slab.get(), *dslab = nullptr;
 	CU_OK(cudaHostGetDevicePointer((void **)&dslab, slab, 0));
 	memset(slab, 0, per_q * num_queues);
 	for (uint32_t q = 0; q < num_queues; q++) {
@@ -288,14 +272,14 @@ static int lun_open_on(const char *ctrlr, int scsi_target_num, int on_device, ui
 		Q.h_cpls = (oimgpu_cpl *)h;
 		Q.d_cpls = (oimgpu_cpl *)d;
 	}
-	CU_OK(cudaHostAlloc((void **)&L->h_door, sizeof(oimgpu_lun::Door) * num_queues, cudaHostAllocMapped));
-	CU_OK(cudaHostGetDevicePointer((void **)&L->d_door, L->h_door, 0));
-	memset((void *)L->h_door, 0, sizeof(oimgpu_lun::Door) * num_queues);
-	CU_OK(cudaHostAlloc((void **)&L->h_flags, 256, cudaHostAllocMapped));
-	CU_OK(cudaHostGetDevicePointer((void **)&L->d_flags, (void *)L->h_flags, 0));
-	memset((void *)L->h_flags, 0, 256);
-	CU_OK(cudaMalloc((void **)&L->d_vq_state, sizeof(VqState) * num_queues));
-	CU_OK(cudaMemsetAsync(L->d_vq_state, 0, sizeof(VqState) * num_queues, L->stream));
+	CU_OK(L->h_door.alloc(L->device, num_queues));
+	CU_OK(cudaHostGetDevicePointer((void **)&L->d_door, L->h_door.get(), 0));
+	memset((void *)L->h_door.get(), 0, sizeof(oimgpu_lun::Door) * num_queues);
+	CU_OK(L->h_flags.alloc(L->device, 64));
+	CU_OK(cudaHostGetDevicePointer((void **)&L->d_flags, (void *)L->h_flags.get(), 0));
+	memset((void *)L->h_flags.get(), 0, 256);
+	CU_OK(L->d_vq_state.alloc(L->device, num_queues));
+	CU_OK(cudaMemsetAsync(L->d_vq_state.get(), 0, sizeof(VqState) * num_queues, L->stream));
 	CU_OK(cudaStreamSynchronize(L->stream));
 	int per_sm = 0;
 	CU_OK(lun_kernels_init(&per_sm));
@@ -303,7 +287,6 @@ static int lun_open_on(const char *ctrlr, int scsi_target_num, int on_device, ui
 	L->grid_cap = L->sm_count * per_sm;
 	int rc = refresh_peers_locked(L.get());
 	if (rc) return rc;
-	if (bp) open_bdev_locked(*bp);
 	g.handles.push_back(L.get());
 	*out = L.release();
 	return 0;
@@ -329,23 +312,14 @@ extern "C" int oimgpu_lun_close(oimgpu_lun *L)
 {
 	if (!L) return -EINVAL;
 	std::lock_guard<std::mutex> lk(g.mu);
+	oimgpu_lun_stop_poller(L);
 	cudaSetDevice(L->device);
-	if (L->poller_active) {
-		L->h_flags[0] = 1;
-		L->poller_active = false;
-	}
 	cudaStreamSynchronize(L->stream);
 	for_each_ctx(L, [&](const std::string &bn, LunCtx *d, LunCtx *) {
 		retire_stats_locked(bn, L->device, d);
 		return 0;
 	});
-	{
-		ParkedPollers parked(L->device, L);	/* other sessions' resident kernels */
-		free_lun_resources(L);
-		g.handles.erase(std::remove(g.handles.begin(), g.handles.end(), L), g.handles.end());
-	}
-	close_bdev_locked(L->bdev);
-	delete L;
+	destroy_session_locked(L);
 	return 0;
 }
 
@@ -420,7 +394,7 @@ static void launch_queue_kernel(oimgpu_lun *L, uint32_t grid, bool shared, bool 
 	if (!shared && !L->any_mirror && vrings_only && !getenv("OIMGPU_NO_VRING_KERNEL")) k = LUN_KERNEL_VRING;
 	else if (shared) k = L->any_mirror ? LUN_KERNEL_SHARED_QUEUE_MIRROR : LUN_KERNEL_SHARED_QUEUE;
 	else k = L->any_mirror ? LUN_KERNEL_QUEUE_MIRROR : LUN_KERNEL_QUEUE;
-	launch_lun_kernel(k, grid, L->stream, L->d_ctx, (KickHeader *)L->d_kick, L->d_desc);
+	launch_lun_kernel(k, grid, L->stream, L->d_ctx.get(), (KickHeader *)L->d_kick.get(), L->d_desc);
 }
 
 /* CTAs share the queues a pass at a time (KickHeader::shared) only while the queues alone cannot fill HBM with one CTA
@@ -435,7 +409,7 @@ static int staged_descs(oimgpu_lun *L, QueueDesc **desc)
 {
 	const int slot = (int)(L->kicks % oimgpu_lun::kKickSlots);
 	if (L->kicks >= (uint64_t)oimgpu_lun::kKickSlots) CU_OK(cudaEventSynchronize(L->kick_ev[slot]));
-	*desc = (QueueDesc *)(L->h_kick[slot] + sizeof(KickHeader));
+	*desc = (QueueDesc *)(L->h_kick[slot].get() + sizeof(KickHeader));
 	return 0;
 }
 
@@ -444,15 +418,15 @@ static int staged_descs(oimgpu_lun *L, QueueDesc **desc)
 static int launch_staged(oimgpu_lun *L, KickHeader kh, uint32_t nd, uint32_t grid, bool shared)
 {
 	const int slot = (int)(L->kicks % oimgpu_lun::kKickSlots);
-	const QueueDesc *desc = (const QueueDesc *)(L->h_kick[slot] + sizeof(KickHeader));
+	const QueueDesc *desc = (const QueueDesc *)(L->h_kick[slot].get() + sizeof(KickHeader));
 	bool vrings_only = true;
 	for (uint32_t k = 0; k < nd; k++) vrings_only &= desc[k].mode == QMODE_VRING;
 	kh.next = grid;		/* queues 0..grid-1 are taken statically by CTA index */
 	kh.nqueues = nd;
 	kh.shared = shared ? 1 : 0;
-	kh.share = shared ? L->d_share : nullptr;
-	memcpy(L->h_kick[slot], &kh, sizeof(kh));
-	CU_OK(cudaMemcpyAsync(L->d_kick, L->h_kick[slot], sizeof(KickHeader) + sizeof(QueueDesc) * nd, cudaMemcpyHostToDevice, L->stream));
+	kh.share = shared ? L->d_share.get() : nullptr;
+	memcpy(L->h_kick[slot].get(), &kh, sizeof(kh));
+	CU_OK(cudaMemcpyAsync(L->d_kick.get(), L->h_kick[slot].get(), sizeof(KickHeader) + sizeof(QueueDesc) * nd, cudaMemcpyHostToDevice, L->stream));
 	CU_OK(cudaEventRecord(L->kick_ev[slot], L->stream));
 	L->kicks++;
 	launch_queue_kernel(L, grid + (kh.dispatcher ? 1 : 0), shared, vrings_only);
@@ -470,7 +444,7 @@ static QueueDesc desc_device_arrays(oimgpu_lun *L, uint32_t q)
 	const Queue &Q = L->queues[q];
 	QueueDesc D;
 	memset(&D, 0, sizeof(D));
-	D.vq_state = L->d_vq_state + q;
+	D.vq_state = L->d_vq_state.get() + q;
 	D.reqs = Q.dev_reqs;
 	D.iovs = Q.dev_iovs;
 	D.cpls = Q.dev_cpls ? Q.dev_cpls : Q.d_cpls;
@@ -488,7 +462,7 @@ static QueueDesc desc_slot_ring(oimgpu_lun *L, uint32_t q)
 	const Queue &Q = L->queues[q];
 	QueueDesc D;
 	memset(&D, 0, sizeof(D));
-	D.vq_state = L->d_vq_state + q;
+	D.vq_state = L->d_vq_state.get() + q;
 	D.reqs = Q.d_reqs;
 	D.iovs = Q.d_iovs;
 	D.cpls = Q.d_cpls;
@@ -504,21 +478,20 @@ static QueueDesc desc_virtqueue(oimgpu_lun *L, uint32_t q)
 	QueueDesc D;
 	memset(&D, 0, sizeof(D));
 	D.mode = QMODE_VRING;
-	D.iovs = L->d_iov_scratch;
+	D.iovs = L->d_iov_scratch.get();
 	D.vq_size = Q.vq_size;
 	D.vq_desc = Q.vq_desc;
 	D.vq_avail = Q.vq_avail;
 	D.vq_used = Q.vq_used;
 	D.vq_in_hbm = Q.vq_in_hbm ? 1 : 0;
-	D.vq_state = L->d_vq_state + q;
+	D.vq_state = L->d_vq_state.get() + q;
 	return D;
 }
 
 /* [grid_cap][32][kIovRow] SG rows for the parser lanes of virtqueue mode */
 static cudaError_t ensure_iov_scratch(oimgpu_lun *L)
 {
-	if (L->d_iov_scratch) return cudaSuccess;
-	return cudaMalloc((void **)&L->d_iov_scratch, sizeof(oimgpu_iov) * (size_t)L->grid_cap * kPass * kIovRow);
+	return L->d_iov_scratch ? cudaSuccess : L->d_iov_scratch.alloc(L->device, (size_t)L->grid_cap * kPass * kIovRow);
 }
 
 extern "C" int oimgpu_kick(oimgpu_lun *L)
@@ -585,12 +558,12 @@ extern "C" int oimgpu_kick(oimgpu_lun *L)
 	}
 	const bool shared = !L->write_hot && may_share_queues(L, nd, grid);
 	if (!shared) grid = std::min(grid, nd);
-	if (shared) CU_OK(cudaMemsetAsync(L->d_share, 0, sizeof(QShare) * nd, L->stream));
+	if (shared) CU_OK(cudaMemsetAsync(L->d_share.get(), 0, sizeof(QShare) * nd, L->stream));
 	KickHeader kh;
 	memset(&kh, 0, sizeof(kh));	/* run-to-completion: persistent = 0 */
 	rc = launch_staged(L, kh, nd, grid, shared);
 	if (rc) return rc;
-	CU_OK(cudaMemcpyAsync((void *)L->h_mix, (const uint8_t *)L->d_ctx + offsetof(LunCtx, mix), sizeof(unsigned long long) * 2,
+	CU_OK(cudaMemcpyAsync((void *)L->h_mix.get(), (const uint8_t *)L->d_ctx.get() + offsetof(LunCtx, mix), sizeof(unsigned long long) * 2,
 			      cudaMemcpyDeviceToHost, L->stream));
 	CU_OK(cudaEventRecord(L->done, L->stream));
 	return (int)nd;
@@ -664,22 +637,13 @@ extern "C" int oimgpu_submit_batch(oimgpu_lun *L, uint32_t nq, uint32_t per_q, c
 	CU_OK(cudaSetDevice(L->device));
 	if (L->bs_pending) return -EAGAIN;
 	const size_t n = (size_t)nq * per_q;
-	if (n > L->bs_cap_reqs || niovs > L->bs_cap_iovs) {
+	if (n > L->bs_d_reqs.size() || n > L->bs_d_cpls.size() || niovs > L->bs_d_iovs.size()) {
 		CU_OK(cudaStreamSynchronize(L->stream));
-		/* growing the staging arrays frees the old ones: see ParkedPollers */
 		std::lock_guard<std::mutex> lk(g.mu);
 		ParkedPollers parked(L->device, L);
-		if (n > L->bs_cap_reqs) {
-			cudaFree(L->bs_d_reqs); cudaFree(L->bs_d_cpls);
-			CU_OK(cudaMalloc((void **)&L->bs_d_reqs, n * sizeof(oimgpu_req)));
-			CU_OK(cudaMalloc((void **)&L->bs_d_cpls, n * sizeof(oimgpu_cpl)));
-			L->bs_cap_reqs = n;
-		}
-		if (niovs > L->bs_cap_iovs) {
-			cudaFree(L->bs_d_iovs);
-			CU_OK(cudaMalloc((void **)&L->bs_d_iovs, (size_t)std::max<uint32_t>(niovs, 1) * sizeof(oimgpu_iov)));
-			L->bs_cap_iovs = niovs;
-		}
+		CU_OK(L->bs_d_reqs.grow(L->device, n, parked));
+		CU_OK(L->bs_d_cpls.grow(L->device, n, parked));
+		CU_OK(L->bs_d_iovs.grow(L->device, niovs, parked));
 	}
 	auto pinned = [](const void *p) {
 		cudaPointerAttributes a;
@@ -690,19 +654,12 @@ extern "C" int oimgpu_submit_batch(oimgpu_lun *L, uint32_t nq, uint32_t per_q, c
 	const bool pin_out = pinned(cpls);
 	const size_t need = (pin_in ? 0 : n * sizeof(oimgpu_req) + (size_t)niovs * sizeof(oimgpu_iov)) +
 			    (pin_out ? 0 : n * sizeof(oimgpu_cpl));
-	if (need > L->bs_h_cap) {
+	if (need > L->bs_h_pin.size()) {
 		CU_OK(cudaStreamSynchronize(L->stream));
-		if (L->bs_h_pin) {
-			/* cudaFreeHost waits for every GPU the memory is mapped into: see ParkedPollers */
-			std::lock_guard<std::mutex> lk(g.mu);
-			ParkedPollers parked(-1, L);
-			cudaFreeHost(L->bs_h_pin);
-		}
-		L->bs_h_pin = nullptr;
-		CU_OK(cudaHostAlloc((void **)&L->bs_h_pin, need, cudaHostAllocDefault));
-		L->bs_h_cap = need;
+		std::lock_guard<std::mutex> lk(g.mu);
+		CU_OK(L->bs_h_pin.grow(L->device, need, ParkedPollers(L->bs_h_pin.waits_for(), L)));
 	}
-	uint8_t *bounce = L->bs_h_pin;
+	uint8_t *bounce = L->bs_h_pin.get();
 	const oimgpu_iov *src_iovs = iovs;
 	const oimgpu_req *src_reqs = reqs;
 	if (!pin_in) {
@@ -714,27 +671,27 @@ extern "C" int oimgpu_submit_batch(oimgpu_lun *L, uint32_t nq, uint32_t per_q, c
 		bounce += n * sizeof(oimgpu_req);
 	}
 	oimgpu_cpl *h_cpls = pin_out ? cpls : (oimgpu_cpl *)bounce;
-	if (niovs) CU_OK(cudaMemcpyAsync(L->bs_d_iovs, src_iovs, (size_t)niovs * sizeof(oimgpu_iov), cudaMemcpyHostToDevice, L->stream));
+	if (niovs) CU_OK(cudaMemcpyAsync(L->bs_d_iovs.get(), src_iovs, (size_t)niovs * sizeof(oimgpu_iov), cudaMemcpyHostToDevice, L->stream));
 	const uint32_t groups = pin_in ? 1 : std::min<uint32_t>(8, nq);
 	int kicked = 0;
 	for (uint32_t g = 0; g < groups; g++) {
 		const uint32_t q0 = (uint32_t)((uint64_t)nq * g / groups), q1 = (uint32_t)((uint64_t)nq * (g + 1) / groups);
 		const size_t r0 = (size_t)q0 * per_q, rn = (size_t)(q1 - q0) * per_q;
 		if (!pin_in) memcpy(const_cast<oimgpu_req *>(src_reqs) + r0, reqs + r0, rn * sizeof(oimgpu_req));
-		CU_OK(cudaMemcpyAsync(L->bs_d_reqs + r0, src_reqs + r0, rn * sizeof(oimgpu_req), cudaMemcpyHostToDevice, L->stream));
+		CU_OK(cudaMemcpyAsync(L->bs_d_reqs.get() + r0, src_reqs + r0, rn * sizeof(oimgpu_req), cudaMemcpyHostToDevice, L->stream));
 		for (uint32_t q = q0; q < q1; q++) {
 			Queue &Q = L->queues[q];
 			if (Q.dev_count) return -EAGAIN;
-			Q.dev_reqs = L->bs_d_reqs + (size_t)q * per_q;
-			Q.dev_iovs = L->bs_d_iovs;
-			Q.dev_cpls = L->bs_d_cpls + (size_t)q * per_q;
+			Q.dev_reqs = L->bs_d_reqs.get() + (size_t)q * per_q;
+			Q.dev_iovs = L->bs_d_iovs.get();
+			Q.dev_cpls = L->bs_d_cpls.get() + (size_t)q * per_q;
 			Q.dev_count = per_q;
 			Q.dev_iov_limit = niovs;
 		}
 		int rc = oimgpu_kick(L);
 		if (rc < 0) return rc;
 		kicked += rc;
-		CU_OK(cudaMemcpyAsync(h_cpls + r0, L->bs_d_cpls + r0, rn * sizeof(oimgpu_cpl), cudaMemcpyDeviceToHost, L->stream));
+		CU_OK(cudaMemcpyAsync(h_cpls + r0, L->bs_d_cpls.get() + r0, rn * sizeof(oimgpu_cpl), cudaMemcpyDeviceToHost, L->stream));
 	}
 	L->bs_user_cpls = pin_out ? nullptr : cpls;
 	L->bs_h_cpls = h_cpls;
@@ -817,16 +774,16 @@ static int read_iostat(oimgpu_lun *L, const LunCtx *d_ctx, oimgpu_iostat *out)
 extern "C" int oimgpu_lun_iostat(oimgpu_lun *L, oimgpu_iostat *out)
 {
 	if (!L || !out) return -EINVAL;
-	return read_iostat(L, L->d_ctx, out);
+	return read_iostat(L, L->d_ctx.get(), out);
 }
 
 extern "C" int oimgpu_lun_target_iostat(oimgpu_lun *L, int scsi_target_num, oimgpu_iostat *out)
 {
 	if (!L || !out || scsi_target_num < 0 || scsi_target_num >= OIMGPU_CTRLR_MAX_DEVS) return -EINVAL;
-	if (scsi_target_num == L->target) return read_iostat(L, L->d_ctx, out);
+	if (scsi_target_num == L->target) return read_iostat(L, L->d_ctx.get(), out);
 	std::lock_guard<std::mutex> lk(g.mu);
 	if (L->peer_bdev[scsi_target_num].empty()) return -ENODEV;
-	return read_iostat(L, L->d_peer[scsi_target_num], out);
+	return read_iostat(L, L->d_peer[scsi_target_num].get(), out);
 }
 
 /* session-visible target state: hot-remove flags (vhost_scsi.c:1093-1100, lun.c:171-176) */
@@ -836,7 +793,7 @@ extern "C" int oimgpu_lun_set_removed(oimgpu_lun *L, int removed, int lun_remove
 	if (int rc = drain_stream(L)) return rc;
 	L->h_ctx.removed = removed != 0;
 	L->h_ctx.lun_removed = lun_removed != 0;
-	CU_OK(h2d_sync(L, L->d_ctx, &L->h_ctx, offsetof(LunCtx, stats)));
+	CU_OK(h2d_sync(L, L->d_ctx.get(), &L->h_ctx, offsetof(LunCtx, stats)));
 	return 0;
 }
 
@@ -855,7 +812,7 @@ extern "C" int oimgpu_lun_set_mem_table(oimgpu_lun *L, const oimgpu_mem_region *
 		L->h_ctx.region[i].size = regions[i].size;
 		L->h_ctx.region[i].addr = regions[i].addr;
 	}
-	CU_OK(h2d_sync(L, L->d_ctx, &L->h_ctx, offsetof(LunCtx, stats)));
+	CU_OK(h2d_sync(L, L->d_ctx.get(), &L->h_ctx, offsetof(LunCtx, stats)));
 	return 0;
 }
 
@@ -870,7 +827,7 @@ extern "C" int oimgpu_vq_attach(oimgpu_lun *L, uint32_t q, const void *desc, con
 	if (int rc = drain_stream(L)) return rc;
 	CU_OK(ensure_iov_scratch(L));
 	VqState st ={ last_avail_idx, last_used_idx, last_avail_idx, 0 };
-	CU_OK(h2d_sync(L, L->d_vq_state + q, &st, sizeof(st)));
+	CU_OK(h2d_sync(L, L->d_vq_state.get() + q, &st, sizeof(st)));
 	Queue &Q = L->queues[q];
 	Q.vq_desc = (const uint8_t *)desc;
 	Q.vq_avail = (const uint8_t *)avail;
@@ -889,7 +846,7 @@ extern "C" int oimgpu_vq_detach(oimgpu_lun *L, uint32_t q, uint16_t *last_avail_
 	std::lock_guard<std::recursive_mutex> hl(L->mu);
 	if (int rc = drain_stream(L)) return rc;
 	VqState st;
-	CU_OK(cudaMemcpy(&st, L->d_vq_state + q, sizeof(st), cudaMemcpyDeviceToHost));
+	CU_OK(cudaMemcpy(&st, L->d_vq_state.get() + q, sizeof(st), cudaMemcpyDeviceToHost));
 	if (last_avail_idx) *last_avail_idx = (uint16_t)st.last_avail;
 	if (last_used_idx) *last_used_idx = (uint16_t)st.last_used;
 	Queue &Q = L->queues[q];
@@ -935,7 +892,7 @@ extern "C" int oimgpu_lun_start_poller(oimgpu_lun *L, uint32_t max_ctas, uint32_
 	if (rc) return rc;
 	uint32_t nd = 0;
 	std::vector<VqState> cursors(L->num_queues);
-	CU_OK(cudaMemcpy(cursors.data(), L->d_vq_state, sizeof(VqState) * L->num_queues, cudaMemcpyDeviceToHost));
+	CU_OK(cudaMemcpy(cursors.data(), L->d_vq_state.get(), sizeof(VqState) * L->num_queues, cudaMemcpyDeviceToHost));
 	for (uint32_t q = 0; q < L->num_queues; q++) {
 		Queue &Q = L->queues[q];
 		if (Q.dev_count || Q.tail != Q.kicked) return -EBUSY;	/* drain pending launches first */
@@ -955,7 +912,7 @@ extern "C" int oimgpu_lun_start_poller(oimgpu_lun *L, uint32_t max_ctas, uint32_
 	/* slot-ring cursors live in the same VqState array (virtqueues keep theirs); the dispatcher's view of
 	 * every doorbell starts at "nothing new" */
 	for (uint32_t q = 0; q < L->num_queues; q++) cursors[q].hint = cursors[q].last_avail;
-	CU_OK(h2d_sync(L, L->d_vq_state, cursors.data(), sizeof(VqState) * L->num_queues));
+	CU_OK(h2d_sync(L, L->d_vq_state.get(), cursors.data(), sizeof(VqState) * L->num_queues));
 	/* worker CTAs + one dispatcher CTA (KickHeader::dispatcher).  With fewer queues than that, the workers share
 	 * the queues a pass at a time: up to a ring's worth of passes per queue can be in flight at once. */
 	uint64_t want = 0;
@@ -978,7 +935,7 @@ extern "C" int oimgpu_lun_start_poller(oimgpu_lun *L, uint32_t max_ctas, uint32_
 			sh[k].base_used = cursors[k].last_used;
 			sh[k].latched = 1;
 		}
-		CU_OK(h2d_sync(L, L->d_share, sh.data(), sizeof(QShare) * nd));
+		CU_OK(h2d_sync(L, L->d_share.get(), sh.data(), sizeof(QShare) * nd));
 	}
 	L->h_flags[0] = 0;
 	L->h_flags[16] = 0;

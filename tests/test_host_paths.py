@@ -1,6 +1,7 @@
 """Host paths of the C ABI next to a resident poller (GPU only): host-array batches through the poller's rings, the
 error codes of that path, and control calls that park and restart the pollers of other sessions.  Every poller arms
 the idle watchdog, and every call that waits for the GPU runs in a daemon thread with a deadline."""
+import ctypes
 import errno
 import threading
 
@@ -132,8 +133,9 @@ def test_poller_host_batch_error_codes(gpu):
 
 @pytest.mark.timeout(180)
 def test_park_sites_keep_a_resident_poller(gpu, oracles):
-    """histogram disable, delete_bdev of an unrelated bdev and mem_unregister park the resident poller of another
-    session and bring it back; afterwards it still serves a trace bit-exactly"""
+    """histogram disable, delete_bdev of an unrelated bdev (with and without a histogram), mem_unregister and a session
+    open that fails with -ENOMEM park the resident poller of another session and bring it back, and bdev_digest of an
+    unrelated bdev on its GPU does not stop it; afterwards it still serves a trace bit-exactly"""
     import torch
     nb, nq, rounds = 1 << 16, 2, 4
     t = traces.partitioned_queues(nq, 32 * rounds, nb, pattern="randrw", read_pct=60, io_blocks=8)
@@ -143,6 +145,9 @@ def test_park_sites_keep_a_resident_poller(gpu, oracles):
     _setup(gpu, "pk0", nb)
     gpu.construct_malloc_bdev(1024, 512, name="pk1", device=0)
     gpu.construct_malloc_bdev(1024, 512, name="pk2", device=0)
+    gpu.construct_malloc_bdev(1024, 512, name="pk3", device=0)
+    gpu.construct_vhost_scsi_controller("pk1.ctl")
+    gpu.add_vhost_scsi_lun("pk1.ctl", 0, "pk1")
     try:
         arena = torch.from_numpy(host.copy()).pin_memory()
         iovs = t.bind(arena.data_ptr())
@@ -158,6 +163,13 @@ def test_park_sites_keep_a_resident_poller(gpu, oracles):
                 _blocking(lambda: gpu.delete_bdev("pk2"))
                 gpu.mem_register(reg)
                 _blocking(lambda: gpu.mem_unregister(reg))
+                gpu.enable_bdev_histogram("pk3", True)
+                _blocking(lambda: gpu.delete_bdev("pk3"))
+                _blocking(lambda: gpu.bdev_digest("pk1"))
+                h = ctypes.c_void_p()
+                # terabytes of kick staging: refused, and the half-open session is taken apart
+                assert _blocking(lambda: gpu.load().oimgpu_lun_open(b"pk1.ctl", 0, 0xFFFFFFFF, 64, ctypes.byref(h))) \
+                    == -errno.ENOMEM
                 assert lun.poller_running()
                 for r in range(rounds):
                     for q in range(nq):
@@ -174,10 +186,48 @@ def test_park_sites_keep_a_resident_poller(gpu, oracles):
                 assert lun.poller_running()
             finally:
                 lun.stop_poller()
-            assert lun.iostat()["kernel_launches"] == 4, "three parks, each followed by a restart"
+            assert lun.iostat()["kernel_launches"] == 6, "five parks, each followed by a restart"
         util.assert_cpls_equal(got, want, t.reqs)
         assert (arena.numpy() == want_arena).all(), "client buffers"
         assert (gpu.bdev_read_raw("pk0", 0, nb * 512) == want_store).all(), "store"
     finally:
         _teardown(gpu, "pk0")
-        gpu.delete_bdev("pk1")
+        _teardown(gpu, "pk1")
+
+
+@pytest.mark.timeout(120)
+def test_session_survives_a_refused_host_batch(gpu, oracles):
+    """a host-array batch whose staging arrays cannot be allocated (128 GiB of request slots) is refused with -ENOMEM
+    before the caller's arrays are read; the same session then serves a batch as the oracle does"""
+    import torch
+    nb, nq, k = 1 << 14, 4, 32
+    t = traces.partitioned_queues(nq, k, nb, pattern="randrw", read_pct=60, io_blocks=8)
+    host = np.zeros(t.arena_bytes, dtype=np.uint8)
+    traces.fill_arena(host, t)
+    with oracles.PortOracle(nb) as o:                          # the same batch, twice
+        o.store[:] = traces.pattern_bytes(7, 0, o.store.size)
+        want_arena = host.copy()
+        want_first = o.submit(t.reqs, t.bind(want_arena.ctypes.data))
+        want = o.submit(t.reqs, t.bind(want_arena.ctypes.data))
+        want_store = o.store.copy()
+    _setup(gpu, "hp2", nb)
+    try:
+        arena = torch.from_numpy(host.copy()).pin_memory()
+        iovs = np.ascontiguousarray(t.bind(arena.data_ptr()))
+        reqs = np.ascontiguousarray(t.reqs)
+        with gpu.Lun("hp2.ctl", 0, num_queues=nq, queue_size=64) as lun:
+            def batch():
+                cpls = np.zeros(len(reqs), dtype=abi.cpl_dtype)
+                rc = _blocking(lambda: gpu.load().oimgpu_submit_and_wait(
+                    lun.h, nq, k, reqs.ctypes.data, iovs.ctypes.data, len(iovs), cpls.ctypes.data, abi.MEM_HOST))
+                assert rc == 0, f"rc {rc}"
+                return cpls
+            util.assert_cpls_equal(batch(), want_first, t.reqs)
+            one = np.zeros(1, dtype=abi.req_dtype)
+            assert _submit_batch(gpu, lun, 1, 1 << 31, one, np.zeros(1, dtype=abi.iov_dtype),
+                                 np.zeros(1, dtype=abi.cpl_dtype)) == -errno.ENOMEM
+            util.assert_cpls_equal(batch(), want, t.reqs)
+        assert (arena.numpy() == want_arena).all(), "client buffers"
+        assert (gpu.bdev_read_raw("hp2", 0, nb * 512) == want_store).all(), "store"
+    finally:
+        _teardown(gpu, "hp2")
