@@ -250,6 +250,44 @@ struct oimgpu_mirror_check {
  * a moment of the race and a repair may undo their writes. */
 int oimgpu_bdev_mirror_check(const char *name, uint64_t offset_blocks, uint64_t num_blocks, int repair,
 			     uint64_t *ranges, uint32_t max_ranges, struct oimgpu_mirror_check *out);
+/* Volume images: a bdev's bytes in a sparse file, and back.  The format is canonical (the same content always gives the
+ * same file, byte for byte) and little-endian:
+ *   header   4096 bytes, zero-padded: char magic[8] = "OIMGPUIM", u32 version = 1, u32 block_size, u64 num_blocks,
+ *            u32 granule_bytes = 4096, u32 reserved = 0, u64 nextents, u64 data_bytes, u64 digest[2], char uuid[36]
+ *            (the source bdev's)
+ *   table    nextents x {u64 offset_bytes, u64 len_bytes}, zero-padded to a multiple of 4096 bytes: the maximal runs of
+ *            4 KiB granules of the store (num_blocks x block_size bytes, whatever the block size) that hold a non-zero
+ *            byte, sorted, neither overlapping nor adjacent; the last run ends at the end of the store when its size is
+ *            not a multiple of 4096
+ *   data     the runs' bytes, concatenated in table order
+ * so the file holds 4096 + round_up(16 x nextents, 4096) + data_bytes bytes.  digest is oimgpu_bdev_digest's over the
+ * whole store, its last word zero-padded when the size is not a multiple of 8.  Neither call counts in the bdev's
+ * iostat or histogram. */
+struct oimgpu_image_info {
+	uint64_t num_blocks, nextents, data_bytes, file_bytes;
+	uint32_t block_size, granule_bytes;
+	char uuid[37];	/* the uuid the image was saved from (not enforced on load) */
+};
+/* Write replica 0 of bdev `name` to a new file `path` (O_CREAT | O_EXCL: never over an existing file), fsync it and
+ * describe it in *out.  A failed save removes the partial file.
+ * Quiescence: as oimgpu_bdev_mirror_check, every session that reaches the bdev (and every session on replica 0's GPU)
+ * is held for the call - resident pollers parked and restarted, launched work waited for - so the image is the volume
+ * between two writes of this process and a guest sees one stall of the call's length.  Writers in another process
+ * (the exporter of an imported replica) are not paused.
+ * -EINVAL NULL argument; -ENODEV no such bdev / control-only; -EEXIST `path` exists; -EBUSY an NBD export or a
+ * block-I/O channel serves the bdev (neither can be paused); -EIO a short write or a GPU failure; other open / write /
+ * fsync errors as -errno. */
+int oimgpu_bdev_image_save(const char *name, const char *path, struct oimgpu_image_info *out);
+/* Fill every replica of bdev `name` with the image at `path`: zero-fill, then the image's runs, then the digest is
+ * recomputed on replica 0 and compared with the header's.  The bdev must not be in use: construct it, load it, then
+ * attach it.  The header, the table and the file's exact size are checked against the bdev's geometry before any store
+ * is touched; the uuid is reported, not enforced, so an image can be restored into a differently named volume.
+ * The sessions on replica 0's GPU are held for the call.
+ * -EINVAL NULL argument, not an image, a geometry other than the bdev's, a malformed table or a file of the wrong size
+ * (the bdev is untouched); -ENODEV no such bdev / control-only; -EBUSY the bdev is open (a session target, an NBD export
+ * or a block-I/O channel); -EIO a short read, a GPU failure, or a digest that does not match after the load - the bdev
+ * then holds the file's bytes and must not be trusted; other open / read errors as -errno. */
+int oimgpu_bdev_image_load(const char *name, const char *path, struct oimgpu_image_info *out);
 int oimgpu_bdev_delete(const char *name);			/* -ENODEV if unknown; attached targets are hot-removed
 								 * (as spdk_bdev_unregister does); -EBUSY while a
 								 * data path (oimgpu_lun) is open on it */

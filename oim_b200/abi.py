@@ -73,6 +73,11 @@ mirror_check_dtype = np.dtype([("blocks_checked", "<u8"), ("mismatched_blocks", 
                                ("nranges", "<u4"), ("truncated", "<u4")])
 assert mirror_check_dtype.itemsize == 32
 
+# volume image of a bdev (oimgpu_bdev_image_save / _load): struct oimgpu_image_info
+image_info_dtype = np.dtype([("num_blocks", "<u8"), ("nextents", "<u8"), ("data_bytes", "<u8"), ("file_bytes", "<u8"),
+                             ("block_size", "<u4"), ("granule_bytes", "<u4"), ("uuid", "S37")], align=True)
+assert image_info_dtype.itemsize == 80
+
 # completion fields the reference defines (everything but our bookkeeping extras)
 CPL_PARITY_FIELDS = ("tag", "sense_len", "resid", "status_qualifier", "status", "response",
                      "sense", "resp_valid", "used_len")

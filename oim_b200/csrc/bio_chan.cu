@@ -93,6 +93,7 @@ extern "C" int oimgpu_bio_chan_open(const char *bdev_name, oimgpu_bio_chan **out
 	CU_OK(cudaSetDevice(c->device));
 	CU_OK(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
 	open_bdev_locked(*b);	/* oimgpu_bdev_delete returns -EBUSY while the channel is open */
+	b->bio_chans++;	/* and an image save: a channel's submissions cannot be paused */
 	*out = c.release();
 	return 0;
 }
@@ -111,6 +112,8 @@ extern "C" int oimgpu_bio_chan_close(oimgpu_bio_chan *c)
 		for (auto &st : c->staging) st.h.reset(parked);
 		for (auto &h : c->retired_staging) h.reset(parked);
 		close_bdev_locked(c->bdev);
+		Bdev *b = find_bdev_locked(c->bdev.c_str());
+		if (b && b->bio_chans > 0) b->bio_chans--;
 	}
 	delete c;
 	return 0;

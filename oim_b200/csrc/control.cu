@@ -468,7 +468,7 @@ static int sync_session_streams_locked()
 
 namespace oimgpu { __global__ void oim_digest_kernel(const uint64_t *p, uint64_t nwords, unsigned long long *out); }
 
-static int digest_locked(int device, const void *dptr, uint64_t nbytes, uint64_t out[2])
+int oimgpu::digest_locked(int device, const void *dptr, uint64_t nbytes, uint64_t out[2])
 {
 	if (!dptr || !out || (nbytes & 7) || ((uintptr_t)dptr & 7)) return -EINVAL;
 	const int slot = find_device_slot(device);

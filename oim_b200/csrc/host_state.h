@@ -1,6 +1,6 @@
 /*
  * host_state.h - what the host-side files of liboimgpu.so (control.cu, session.cu, nbd.cu, copy_chan.cu, bio_chan.cu,
- * mirror_check.cu) share: the registry, the session, the helpers more than one of them calls, the Buf that owns device and
+ * mirror_check.cu, bdev_image.cu) share: the registry, the session, the helpers more than one of them calls, the Buf that owns device and
  * pinned memory and frees it only under a ParkedPollers scope, and the channels' EventFifo.  Internal, not installed.
  */
 #pragma once
@@ -148,6 +148,7 @@ struct Bdev {
 	uint32_t block_size = 0;
 	int opens = 0;		/* open_bdev_locked: session targets (own and peer), NBD exports, bio channels */
 	int nbd_exports = 0;	/* oimgpu_nbd_serve calls serving it (also counted in opens) */
+	int bio_chans = 0;	/* block-I/O channels open on it (also counted in opens) */
 	std::vector<Replica> replicas;
 	Buf<unsigned long long, Mem::Device> hist;	/* enable_bdev_histogram: kHistBuckets counters on replica 0's GPU */
 	unsigned long long retired[12] = {};	/* counters of sessions that are gone (same layout as LunCtx::stats) */
@@ -221,6 +222,8 @@ void refresh_ctrlr_sessions_locked(const std::string &ctrlr);
 int publish_ctx_locked(const std::string &bdev, size_t offset, const void *value, size_t len);	/* every LunCtx of the bdev */
 cudaError_t launch_copy(cudaStream_t st, int sm_count, void *dst, const void *src, uint64_t nbytes);
 cudaError_t launch_fill(cudaStream_t st, int sm_count, void *dst, uint8_t fill, uint64_t nbytes);
+/* oimgpu_digest_device on the device's housekeeping stream; caller holds g.mu */
+int digest_locked(int device, const void *dptr, uint64_t nbytes, uint64_t out[2]);
 void unpin_all_host_ranges();	/* oimgpu_mem_ensure's registrations */
 bool host_range_pinned(const void *addr, size_t len);	/* inside one range the library pinned or registered (no driver call) */
 int pin_host_pages(const void *addr, size_t len);	/* pin what of the pages is not pinned yet; -EFAULT */

@@ -10,7 +10,8 @@
  *   vhost methods        S/lib/vhost/vhost_rpc.c:65-478
  * and is pinned against the reference's own server running in-process (tests/test_rpc_daemon.py).  Four methods are the
  * project's own, for mirrored bdevs: construct_mirror_bdev, export_bdev_store, check_mirror_bdev and
- * replace_mirror_replica (INTEGRATION.md 3c).
+ * replace_mirror_replica (INTEGRATION.md 3c); two more, save_bdev_image and load_bdev_image, move any bdev's bytes to
+ * and from a sparse image file (INTEGRATION.md 3d).
  *
  * CLI as S/app/vhost/vhost.c:43-48 + S/lib/event/app.c:826-960:
  *   -S <dir> vhost socket directory   -r <path> RPC socket (default /var/tmp/spdk.sock)
@@ -589,6 +590,19 @@ static Reply dispatch(const std::string &method, const Json *params, const Json 
 		int rc = oimgpu_bdev_mirror_replace_remote(a->raw.c_str(), rep, h.data());
 		if (rc < 0) return error(id, E_INVALID_PARAMS, strerr(rc));
 		return result(id, "true");
+	}
+	if (method == "save_bdev_image" || method == "load_bdev_image") {
+		/* a bdev's bytes to a new image file, or an image into a bdev nothing has open yet; not part of the
+		 * configuration dump, since an image is data, not state */
+		if (!decode(params, {{"name", Json::Str, false, &a}, {"path", Json::Str, false, &b}})) return bad;
+		oimgpu_image_info info;
+		int rc = method == "save_bdev_image" ? oimgpu_bdev_image_save(a->raw.c_str(), b->raw.c_str(), &info)
+						     : oimgpu_bdev_image_load(a->raw.c_str(), b->raw.c_str(), &info);
+		if (rc < 0) return error(id, E_INVALID_PARAMS, strerr(rc));
+		return result(id, "{\"name\":" + jstr(a->raw) + ",\"path\":" + jstr(b->raw) +
+				  ",\"block_size\":" + std::to_string(info.block_size) + ",\"num_blocks\":" + std::to_string(info.num_blocks) +
+				  ",\"uuid\":" + jstr(info.uuid) + ",\"extents\":" + std::to_string(info.nextents) +
+				  ",\"data_bytes\":" + std::to_string(info.data_bytes) + ",\"file_bytes\":" + std::to_string(info.file_bytes) + "}");
 	}
 	if (method == "delete_bdev") {
 		if (!decode(params, {{"name", Json::Str, false, &a}})) return bad;

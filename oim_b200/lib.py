@@ -71,6 +71,8 @@ SYMBOLS = [
     ("oimgpu_bdev_digest", _I, [C.c_char_p, _I, _U64, _U64, C.POINTER(C.c_uint64)]),
     ("oimgpu_digest_device", _I, [_I, _VP, _U64, C.POINTER(C.c_uint64)]),
     ("oimgpu_bdev_mirror_check", _I, [C.c_char_p, _U64, _U64, _I, _VP, _U32, _VP]),
+    ("oimgpu_bdev_image_save", _I, [C.c_char_p, C.c_char_p, _VP]),
+    ("oimgpu_bdev_image_load", _I, [C.c_char_p, C.c_char_p, _VP]),
     ("oimgpu_bdev_delete", _I, [C.c_char_p]),
     ("oimgpu_bdev_get", _I, [C.c_char_p, C.POINTER(BdevInfo)]),
     ("oimgpu_bdev_list", _I, [C.POINTER(BdevInfo), _I]),
@@ -281,6 +283,26 @@ def mirror_check(name: str, offset_blocks: int = 0, num_blocks: int | None = Non
     return {"blocks_checked": int(o["blocks_checked"]), "mismatched_blocks": int(o["mismatched_blocks"]),
             "repaired_blocks": int(o["repaired_blocks"]),
             "ranges": [(int(ranges[2 * i]), int(ranges[2 * i + 1])) for i in range(n)], "truncated": bool(o["truncated"])}
+
+
+def _image_call(fn, what: str, name: str, path) -> dict:
+    out = np.zeros(1, dtype=abi.image_info_dtype)
+    _chk(fn(_b(name), os.fsencode(path), out.ctypes.data), what)
+    o = out[0]
+    return {"num_blocks": int(o["num_blocks"]), "block_size": int(o["block_size"]), "granule_bytes": int(o["granule_bytes"]),
+            "nextents": int(o["nextents"]), "data_bytes": int(o["data_bytes"]), "file_bytes": int(o["file_bytes"]),
+            "uuid": bytes(o["uuid"]).split(b"\0", 1)[0].decode()}
+
+
+def bdev_image_save(name: str, path) -> dict:
+    """write bdev `name`'s bytes to the new sparse image file `path` with its sessions held; the image's geometry,
+    extent count, sizes and source uuid (include/oimgpu.h oimgpu_bdev_image_save)"""
+    return _image_call(load().oimgpu_bdev_image_save, "bdev_image_save", name, path)
+
+
+def bdev_image_load(name: str, path) -> dict:
+    """fill every replica of the unused bdev `name` from the image file `path` (include/oimgpu.h oimgpu_bdev_image_load)"""
+    return _image_call(load().oimgpu_bdev_image_load, "bdev_image_load", name, path)
 
 
 def delete_bdev(name: str) -> None:

@@ -5,9 +5,15 @@ load_config do for the reference: `save` asks every subsystem for the calls that
 {"subsystems": [{"subsystem": ..., "config": [{"method", "params"}, ...]}, ...]}; `load` replays them in order.
   python tools/oimcfg.py save /var/tmp/spdk.sock > cfg.json
   python tools/oimcfg.py load /var/tmp/spdk.sock < cfg.json
+With --images DIR, `save` also writes every bdev's bytes to DIR/<bdev>.img (save_bdev_image), and `load` fills each bdev
+it constructs from DIR/<bdev>.img (load_bdev_image) before the vhost subsystem attaches anything to it:
+  python tools/oimcfg.py save /var/tmp/spdk.sock --images /var/lib/oim/images > cfg.json
+  python tools/oimcfg.py load /var/tmp/spdk.sock --images /var/lib/oim/images < cfg.json
+An image file is never overwritten: save into an empty directory.
 set_bdev_options is a start-up option of SPDK's bdev_io pools (no such pools here): it is saved for fidelity and
 skipped on load."""
 import json
+import os
 import socket
 import sys
 
@@ -36,28 +42,47 @@ class Rpc:
         return rep["result"]
 
 
-def save(rpc: Rpc) -> dict:
-    return {"subsystems": [{"subsystem": s["subsystem"], "config": rpc.call("get_subsystem_config", {"name": s["subsystem"]})}
-                           for s in rpc.call("get_subsystems")]}
+def image_path(images: str, bdev: str) -> str:
+    return os.path.join(os.path.abspath(images), bdev + ".img")
 
 
-def load(rpc: Rpc, cfg: dict) -> int:
+def save(rpc: Rpc, images: str | None = None) -> dict:
+    cfg = {"subsystems": [{"subsystem": s["subsystem"], "config": rpc.call("get_subsystem_config", {"name": s["subsystem"]})}
+                          for s in rpc.call("get_subsystems")]}
+    if images is not None:
+        for b in rpc.call("get_bdevs"):
+            rpc.call("save_bdev_image", {"name": b["name"], "path": image_path(images, b["name"])})
+    return cfg
+
+
+def load(rpc: Rpc, cfg: dict, images: str | None = None) -> int:
     n = 0
     for sub in cfg["subsystems"]:
+        made = []
         for item in sub["config"] or []:
             if item["method"] == "set_bdev_options":
                 continue
-            rpc.call(item["method"], item.get("params"))
+            res = rpc.call(item["method"], item.get("params"))
+            if sub["subsystem"] == "bdev" and item["method"].startswith("construct_"):
+                made.append(res)        # the constructors answer with the bdev's name
             n += 1
+        # the images go in before any later subsystem opens the bdevs
+        for name in made if images is not None else []:
+            rpc.call("load_bdev_image", {"name": name, "path": image_path(images, name)})
     return n
 
 
 if __name__ == "__main__":
-    if len(sys.argv) != 3 or sys.argv[1] not in ("save", "load"):
+    args = sys.argv[1:]
+    images = None
+    if len(args) == 4 and args[2] == "--images":
+        images = args[3]
+        args = args[:2]
+    if len(args) != 2 or args[0] not in ("save", "load"):
         sys.exit(__doc__)
-    r = Rpc(sys.argv[2])
-    if sys.argv[1] == "save":
-        json.dump(save(r), sys.stdout, indent=2)
+    r = Rpc(args[1])
+    if args[0] == "save":
+        json.dump(save(r, images), sys.stdout, indent=2)
         print()
     else:
-        print(f"{load(r, json.load(sys.stdin))} calls replayed", file=sys.stderr)
+        print(f"{load(r, json.load(sys.stdin), images)} calls replayed", file=sys.stderr)
