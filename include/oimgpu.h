@@ -288,6 +288,44 @@ int oimgpu_bdev_image_save(const char *name, const char *path, struct oimgpu_ima
  * or a block-I/O channel); -EIO a short read, a GPU failure, or a digest that does not match after the load - the bdev
  * then holds the file's bytes and must not be trusted; other open / read errors as -errno. */
 int oimgpu_bdev_image_load(const char *name, const char *path, struct oimgpu_image_info *out);
+/* Incremental images (deltas): the granules that changed since a tracked bdev's last save or load, and back.  The format
+ * is canonical (the same parent and current content always give the same bytes) and little-endian:
+ *   header   4096 bytes, zero-padded; its first 100 bytes have the image header's layout with magic "OIMGPUDL",
+ *            version = 1 and digest = the whole-store digest after the delta is applied; then u32 reserved2 = 0 at byte
+ *            100, u64 parent_digest[2] (the digest of the store the delta applies to) at 104, u64 zero_bytes at 120
+ *   table    nextents x {u64 offset_bytes, u64 len}, zero-padded to a multiple of 4096 bytes: the maximal runs of 4 KiB
+ *            granules whose bytes differ from the parent's, split by kind.  Bit 63 of len set: a zero run (its granules
+ *            are now all zero); clear: a data run (each of its granules holds a non-zero byte).  The other bits are the
+ *            run's length in bytes.  Sorted and never overlapping; two runs touch only when their kinds differ; the last
+ *            run ends at the end of the store when its size is not a multiple of 4096
+ *   data     the bytes of the data runs, concatenated in table order (zero runs take none)
+ * so the file holds 4096 + round_up(16 x nextents, 4096) + data_bytes bytes.  oimgpu_bdev_image_load refuses it. */
+struct oimgpu_image_delta_info {
+	uint64_t num_blocks, nextents, data_bytes, zero_bytes, file_bytes;
+	uint64_t parent_digest[2], digest[2];
+	uint32_t block_size, granule_bytes;
+	char uuid[37];
+};
+/* Track bdev `name`'s content for deltas (enable != 0), or stop.  Tracking keeps two tables of a 128-bit fingerprint per
+ * 4 KiB granule on replica 0's GPU (1/128 of the volume together); the baseline a delta is taken against is the
+ * content of the last successful oimgpu_bdev_image_save, _load, _save_delta or _apply_delta.  Enabling allocates the
+ * tables with no baseline yet (enabling again keeps the baseline); disabling frees them.  Guest writes cost nothing
+ * more: a save compares fingerprints of the whole store, so it also sees writes no session of this process made.
+ * -ENODEV no such bdev / control-only; -ENOMEM the tables do not fit. */
+int oimgpu_bdev_image_track(const char *name, int enable);
+/* Write the granules of tracked bdev `name` that changed since its baseline to a new delta file `path`, under
+ * oimgpu_bdev_image_save's rules (O_EXCL, fsync, the partial file removed on failure, the same sessions held).  On
+ * success the saved content becomes the baseline; a failed save keeps the old one.
+ * -ENODATA the bdev is not tracked or has no baseline yet; other errors as oimgpu_bdev_image_save. */
+int oimgpu_bdev_image_save_delta(const char *name, const char *path, struct oimgpu_image_delta_info *out);
+/* Apply the delta at `path` to every replica of bdev `name`, under oimgpu_bdev_image_load's rules (-EBUSY while the bdev
+ * is open; header, table and exact file size checked against its geometry before any store is touched, -EINVAL).  Then
+ * every replica's digest must equal parent_digest, or the call answers -ESTALE with the bdev untouched: a delta applies
+ * only to the content it was taken from, and never to a mirror whose replicas have drifted apart.  The data runs are
+ * written and the zero runs zeroed in every replica, and the digest of replica 0 is checked (-EIO on a mismatch: the
+ * bdev must not be trusted).  A tracked bdev's baseline becomes the result, or is dropped if the call failed after
+ * touching the store.  The bdev need not be tracked. */
+int oimgpu_bdev_image_apply_delta(const char *name, const char *path, struct oimgpu_image_delta_info *out);
 int oimgpu_bdev_delete(const char *name);			/* -ENODEV if unknown; attached targets are hot-removed
 								 * (as spdk_bdev_unregister does); -EBUSY while a
 								 * data path (oimgpu_lun) is open on it */

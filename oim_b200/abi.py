@@ -78,6 +78,12 @@ image_info_dtype = np.dtype([("num_blocks", "<u8"), ("nextents", "<u8"), ("data_
                              ("block_size", "<u4"), ("granule_bytes", "<u4"), ("uuid", "S37")], align=True)
 assert image_info_dtype.itemsize == 80
 
+# incremental image of a tracked bdev (oimgpu_bdev_image_save_delta / _apply_delta): struct oimgpu_image_delta_info
+image_delta_info_dtype = np.dtype([("num_blocks", "<u8"), ("nextents", "<u8"), ("data_bytes", "<u8"), ("zero_bytes", "<u8"),
+                                   ("file_bytes", "<u8"), ("parent_digest", "<u8", (2,)), ("digest", "<u8", (2,)),
+                                   ("block_size", "<u4"), ("granule_bytes", "<u4"), ("uuid", "S37")], align=True)
+assert image_delta_info_dtype.itemsize == 120
+
 # completion fields the reference defines (everything but our bookkeeping extras)
 CPL_PARITY_FIELDS = ("tag", "sense_len", "resid", "status_qualifier", "status", "response",
                      "sense", "resp_valid", "used_len")

@@ -12,8 +12,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "liboimgpu.so")
-SOURCES = ["control.cu", "session.cu", "nbd.cu", "copy_chan.cu", "bio_chan.cu", "mirror_check.cu", "bdev_image.cu", "lun_kernel.cu"]
-HEADERS = ["host_state.h", "lun_kernel.cuh", os.path.join(ROOT, "include", "oimgpu.h")]
+SOURCES = ["control.cu", "session.cu", "nbd.cu", "copy_chan.cu", "bio_chan.cu", "mirror_check.cu", "bdev_image.cu", "image_delta.cu",
+           "lun_kernel.cu"]
+HEADERS = ["host_state.h", "bdev_image.h", "lun_kernel.cuh", os.path.join(ROOT, "include", "oimgpu.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC,-Wall", "-shared", "-I", os.path.join(ROOT, "include"), "-I", CSRC]

@@ -13,13 +13,10 @@
 #include <sys/stat.h>
 #include <unistd.h>
 
-#include "host_state.h"
+#include "bdev_image.h"
 
 namespace {
 
-constexpr int kImageThreads = 256;
-constexpr uint32_t kGranule = 4096;			/* the image's unit of sparseness, independent of the block size */
-constexpr uint64_t kHeaderBytes = 4096;
 constexpr uint64_t kChunkBytes = 64ull << 20;		/* payload per staging chunk (two in flight) */
 constexpr uint32_t kImageVersion = 1;
 constexpr char kImageMagic[8] = {'O', 'I', 'M', 'G', 'P', 'U', 'I', 'M'};
@@ -38,9 +35,6 @@ static_assert(offsetof(ImageHeader, num_blocks) == 16 && offsetof(ImageHeader, n
 	      offsetof(ImageHeader, digest) == 48 && offsetof(ImageHeader, uuid) == 64,
 	      "image header layout");
 
-/* an extent and where its bytes sit in the image's data section */
-struct ImageSeg { uint64_t store_off, data_off, len; };
-
 struct ImageScan {
 	const uint8_t *store;
 	uint64_t nbytes;
@@ -56,18 +50,6 @@ struct ImageMove {
 	const ImageSeg *segs;
 	uint64_t nsegs, begin, end;
 };
-
-/* the bytes of v at and after byte `keep` (1..15) cleared */
-__device__ __forceinline__ void keep_low_bytes(int4 &v, uint32_t keep)
-{
-	int *w = &v.x;
-#pragma unroll
-	for (int j = 0; j < 4; j++) {
-		const uint32_t lo = 4 * j;
-		if (keep <= lo) w[j] = 0;
-		else if (keep < lo + 4) w[j] &= (int)((1u << (8 * (keep - lo))) - 1);
-	}
-}
 
 }  // namespace
 
@@ -131,25 +113,18 @@ oim_image_move_kernel(const __grid_constant__ ImageMove a)
 	}
 }
 
-namespace {
-
-/* page-aligned, page-rounded host memory: a pageable copy that shared a page with a range this process registered
- * would be refused by the driver (mirror_check.cu) */
-using HostPages = std::unique_ptr<uint8_t, decltype(&free)>;
-HostPages host_pages(size_t n)
+HostPages oimgpu::host_pages(size_t n)
 {
 	return HostPages((uint8_t *)aligned_alloc(4096, std::max<size_t>(4096, (n + 4095) & ~(size_t)4095)), &free);
 }
 
-uint64_t table_bytes(uint64_t nextents) { return (16 * nextents + 4095) & ~4095ull; }
-
-uint32_t grid_for(const Device &dev, uint64_t warps_of_work)
+uint32_t oimgpu::grid_for(const Device &dev, uint64_t warps_of_work)
 {
 	const uint64_t per_cta = kImageThreads / 32;
 	return (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((warps_of_work + per_cta - 1) / per_cta, (uint64_t)dev.sm_count * 8));
 }
 
-int write_all(int fd, const uint8_t *p, uint64_t n, uint64_t off)
+int oimgpu::write_all(int fd, const uint8_t *p, uint64_t n, uint64_t off)
 {
 	while (n) {
 		const ssize_t w = pwrite(fd, p, std::min<uint64_t>(n, 1ull << 30), (off_t)off);
@@ -161,7 +136,7 @@ int write_all(int fd, const uint8_t *p, uint64_t n, uint64_t off)
 	return 0;
 }
 
-int read_all(int fd, uint8_t *p, uint64_t n, uint64_t off)
+int oimgpu::read_all(int fd, uint8_t *p, uint64_t n, uint64_t off)
 {
 	while (n) {
 		const ssize_t r = pread(fd, p, std::min<uint64_t>(n, 1ull << 30), (off_t)off);
@@ -173,18 +148,18 @@ int read_all(int fd, uint8_t *p, uint64_t n, uint64_t off)
 	return 0;
 }
 
-/* oimgpu_bdev_digest of the whole store: the words the GPU can read whole, then the last bytes zero-padded to a word */
-int store_digest(const Bdev &b, uint64_t out[2])
+/* the words the GPU can read whole, then the last bytes zero-padded to a word */
+int oimgpu::store_digest(const Bdev &b, size_t r, uint64_t out[2])
 {
-	const Replica &r0 = b.replicas[0];
+	const Replica &rep = b.replicas[r];
 	const uint64_t size = b.num_blocks * (uint64_t)b.block_size, whole = size & ~7ull;
-	if (int rc = digest_locked(r0.device, r0.store, whole, out)) return rc;
+	if (int rc = digest_locked(rep.device, rep.store, whole, out)) return rc;
 	if (size == whole) return 0;
 	HostPages tail = host_pages(8);
 	if (!tail) return -ENOMEM;
 	memset(tail.get(), 0, 8);
-	cudaStream_t st = g.devices[find_device_slot(r0.device)].util;
-	CU_OK(cudaMemcpyAsync(tail.get(), r0.store + whole, size - whole, cudaMemcpyDeviceToHost, st));
+	cudaStream_t st = g.devices[find_device_slot(rep.device)].util;
+	CU_OK(cudaMemcpyAsync(tail.get(), rep.store + whole, size - whole, cudaMemcpyDeviceToHost, st));
 	CU_OK(cudaStreamSynchronize(st));
 	uint64_t w, i = whole / 8;
 	memcpy(&w, tail.get(), 8);
@@ -195,6 +170,8 @@ int store_digest(const Bdev &b, uint64_t out[2])
 	out[1] += z ^ (z >> 31);
 	return 0;
 }
+
+namespace {
 
 void fill_info(const ImageHeader &h, oimgpu_image_info *out)
 {
@@ -208,9 +185,9 @@ void fill_info(const ImageHeader &h, oimgpu_image_info *out)
 	memcpy(out->uuid, h.uuid, sizeof(h.uuid));
 }
 
-/* The image's data section through the staging chunks: save gathers replica 0's extents into a chunk and writes it at
- * file offset data_pos; load reads a chunk and scatters it into every replica.  Caller holds g.mu and the sessions. */
-int move_data(const Bdev &b, const std::vector<ImageSeg> &segs, uint64_t data_bytes, int fd, uint64_t data_pos, bool load)
+}  // namespace
+
+int oimgpu::move_data(const Bdev &b, const std::vector<ImageSeg> &segs, uint64_t data_bytes, int fd, uint64_t data_pos, bool load)
 {
 	if (!data_bytes) return 0;
 	const int dev0 = b.replicas[0].device;
@@ -292,7 +269,35 @@ int move_data(const Bdev &b, const std::vector<ImageSeg> &segs, uint64_t data_by
 	return rc;
 }
 
-/* the granules of replica 0 that hold a non-zero byte, as extents in store order (collect_ranges' walk over a bitmap) */
+namespace {
+
+/* the runs of set bits of a granule bitmap, as extents in store order (collect_ranges' walk over a bitmap) */
+void extents_of(const uint32_t *bits, uint64_t size, std::vector<ImageSeg> &segs, uint64_t *data_bytes)
+{
+	const uint64_t ngran = (size + kGranule - 1) / kGranule;
+	uint64_t start = 0, data = 0;
+	bool in_run = false;
+	auto emit = [&](uint64_t end_gran) {
+		const uint64_t off = start * kGranule, len = std::min(end_gran * kGranule, size) - off;
+		segs.push_back({off, data, len});
+		data += len;
+	};
+	for (uint64_t w = 0; w < (ngran + 31) / 32; w++) {
+		const uint32_t x = bits[w];
+		if (x == (in_run ? 0xffffffffu : 0u)) continue;
+		for (int i = 0; i < 32; i++) {
+			const bool set = x >> i & 1;
+			if (set == in_run) continue;
+			if (set) start = w * 32 + i;
+			else emit(w * 32 + i);
+			in_run = set;
+		}
+	}
+	if (in_run) emit(ngran);	/* bits past ngran are never set */
+	*data_bytes = data;
+}
+
+/* the granules of replica 0 that hold a non-zero byte, as extents in store order */
 int scan_extents(const Bdev &b, std::vector<ImageSeg> &segs, uint64_t *data_bytes)
 {
 	const Replica &r0 = b.replicas[0];
@@ -318,37 +323,25 @@ int scan_extents(const Bdev &b, std::vector<ImageSeg> &segs, uint64_t *data_byte
 		(void)cudaGetLastError();
 		return -EIO;
 	}
-	const uint32_t *bits = (const uint32_t *)h_bits.get();
-	uint64_t start = 0, data = 0;
-	bool in_run = false;
-	auto emit = [&](uint64_t end_gran) {
-		const uint64_t off = start * kGranule, len = std::min(end_gran * kGranule, size) - off;
-		segs.push_back({off, data, len});
-		data += len;
-	};
-	for (uint64_t w = 0; w < (ngran + 31) / 32; w++) {
-		const uint32_t x = bits[w];
-		if (x == (in_run ? 0xffffffffu : 0u)) continue;
-		for (int i = 0; i < 32; i++) {
-			const bool set = x >> i & 1;
-			if (set == in_run) continue;
-			if (set) start = w * 32 + i;
-			else emit(w * 32 + i);
-			in_run = set;
-		}
-	}
-	if (in_run) emit(ngran);	/* bits past ngran are never set */
-	*data_bytes = data;
+	extents_of((const uint32_t *)h_bits.get(), size, segs, data_bytes);
 	return 0;
 }
 
-int save_locked(const Bdev &b, int fd, oimgpu_image_info *out)
+/* ts: a tracked bdev's scan, whose table becomes the baseline once the file is on disk */
+int save_locked(const Bdev &b, int fd, oimgpu_image_info *out, TrackScan *ts)
 {
 	std::vector<ImageSeg> segs;
 	ImageHeader h;
 	memset(&h, 0, sizeof(h));
-	if (int rc = scan_extents(b, segs, &h.data_bytes)) return rc;
-	if (int rc = store_digest(b, h.digest)) return rc;
+	if (tracked(b)) {
+		/* the tracking scan finds the non-zero granules and the digest in the one pass it makes anyway */
+		if (int rc = track_scan_locked(b, false, ts)) return rc;
+		extents_of(ts->nonzero, b.num_blocks * (uint64_t)b.block_size, segs, &h.data_bytes);
+		memcpy(h.digest, ts->digest, sizeof(h.digest));
+	} else {
+		if (int rc = scan_extents(b, segs, &h.data_bytes)) return rc;
+		if (int rc = store_digest(b, 0, h.digest)) return rc;
+	}
 	memcpy(h.magic, kImageMagic, sizeof(h.magic));
 	h.version = kImageVersion;
 	h.block_size = b.block_size;
@@ -404,7 +397,7 @@ int read_image_meta(const Bdev &b, int fd, ImageHeader *h, std::vector<ImageSeg>
 	return data == h->data_bytes ? 0 : -EINVAL;
 }
 
-int load_locked(const Bdev &b, int fd, oimgpu_image_info *out)
+int load_locked(Bdev &b, int fd, oimgpu_image_info *out)
 {
 	ImageHeader h;
 	std::vector<ImageSeg> segs;
@@ -414,15 +407,18 @@ int load_locked(const Bdev &b, int fd, oimgpu_image_info *out)
 	ParkedPollers held(dev0);
 	const Device &dev = g.devices[find_device_slot(dev0)];
 	const uint64_t size = b.num_blocks * (uint64_t)b.block_size;
-	CU_OK(cudaSetDevice(dev0));
-	for (const Replica &r : b.replicas) CU_OK(launch_fill(dev.util, dev.sm_count, r.store, 0, size));
-	if (int rc = move_data(b, segs, h.data_bytes, fd, kHeaderBytes + table_bytes(h.nextents), true)) return rc;
-	uint64_t d[2];
-	if (int rc = store_digest(b, d)) return rc;
-	if (d[0] != h.digest[0] || d[1] != h.digest[1]) {
-		fprintf(stderr, "oimgpu: image loaded into %s does not match its digest\n", b.name.c_str());
-		return -EIO;
+	cudaError_t e = cudaSetDevice(dev0);
+	for (const Replica &r : b.replicas) {
+		if (e == cudaSuccess) e = launch_fill(dev.util, dev.sm_count, r.store, 0, size);
 	}
+	int rc = 0;
+	if (e != cudaSuccess) {
+		fprintf(stderr, "oimgpu: image load into %s failed: %s\n", b.name.c_str(), cudaGetErrorString(e));
+		(void)cudaGetLastError();
+		rc = -EIO;
+	}
+	if (!rc) rc = move_data(b, segs, h.data_bytes, fd, kHeaderBytes + table_bytes(h.nextents), true);
+	if ((rc = finish_load_locked(b, rc, h.digest))) return rc;
 	fill_info(h, out);
 	return 0;
 }
@@ -441,16 +437,18 @@ extern "C" int oimgpu_bdev_image_save(const char *name, const char *path, oimgpu
 	const int fd = open(path, O_WRONLY | O_CREAT | O_EXCL | O_CLOEXEC, 0644);
 	if (fd < 0) return -errno;
 	int rc;
+	TrackScan ts;
 	{
 		/* as oimgpu_bdev_mirror_check: every session that reaches the bdev, and every session on replica 0's GPU,
 		 * held and drained for the whole call, so the image is the volume between two writes of this process */
 		ParkedPollers held(b->replicas[0].device, b->name);
 		rc = held.drain();
-		if (!rc) rc = save_locked(*b, fd, out);
+		if (!rc) rc = save_locked(*b, fd, out, &ts);
 	}
 	if (!rc && fsync(fd)) rc = -errno;
 	if (close(fd) && !rc) rc = -errno;
 	if (rc) unlink(path);
+	else if (tracked(*b)) track_commit_locked(*b, ts.digest);
 	return rc;
 }
 

@@ -77,8 +77,9 @@ static void release_store(const Replica &r)
 }
 
 /* Take a bdev apart once nothing uses it: own stores are freed (their bytes given back to their GPU's count, which
- * places later bdevs), imported ones closed, the histogram freed and the name unregistered.  The pollers of each
- * replica's GPU are parked around its release; the histogram goes with replica 0, on whose GPU it lives. */
+ * places later bdevs), imported ones closed, the histogram and fingerprint tables freed and the name unregistered.
+ * The pollers of each replica's GPU are parked around its release; the histogram and the tables go with replica 0, on
+ * whose GPU they live. */
 static void drop_bdev_locked(Bdev *b)
 {
 	if (!g.control_only) {
@@ -87,6 +88,7 @@ static void drop_bdev_locked(Bdev *b)
 				ParkedPollers parked(r.device);
 				release_store(r);
 				b->hist.reset(parked);
+				for (auto &t : b->track) t.reset(parked);
 			}
 			if (!r.imported) g.devices[find_device_slot(r.device)].bytes_allocated -= b->num_blocks * (uint64_t)b->block_size;
 		}

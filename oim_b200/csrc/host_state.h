@@ -1,6 +1,6 @@
 /*
  * host_state.h - what the host-side files of liboimgpu.so (control.cu, session.cu, nbd.cu, copy_chan.cu, bio_chan.cu,
- * mirror_check.cu, bdev_image.cu) share: the registry, the session, the helpers more than one of them calls, the Buf that owns device and
+ * mirror_check.cu, bdev_image.cu, image_delta.cu) share: the registry, the session, the helpers more than one of them calls, the Buf that owns device and
  * pinned memory and frees it only under a ParkedPollers scope, and the channels' EventFifo.  Internal, not installed.
  */
 #pragma once
@@ -151,6 +151,14 @@ struct Bdev {
 	int bio_chans = 0;	/* block-I/O channels open on it (also counted in opens) */
 	std::vector<Replica> replicas;
 	Buf<unsigned long long, Mem::Device> hist;	/* enable_bdev_histogram: kHistBuckets counters on replica 0's GPU */
+	/* oimgpu_bdev_image_track: two tables of a 128-bit fingerprint per 4 KiB granule on replica 0's GPU.  track[track_base]
+	 * is the content of the last save or load when has_base (base_digest: its whole-store digest); a scan writes the
+	 * other, which becomes the baseline only when its call succeeds */
+	Buf<ulonglong2, Mem::Device> track[2];
+	int track_base = 0;
+	bool has_base = false;
+	uint64_t base_digest[2] = {0, 0};
+	uint64_t track_key[2] = {0, 0};	/* the fingerprint's random key, drawn when the tables are allocated */
 	unsigned long long retired[12] = {};	/* counters of sessions that are gone (same layout as LunCtx::stats) */
 };
 

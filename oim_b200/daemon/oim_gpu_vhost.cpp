@@ -11,7 +11,8 @@
  * and is pinned against the reference's own server running in-process (tests/test_rpc_daemon.py).  Four methods are the
  * project's own, for mirrored bdevs: construct_mirror_bdev, export_bdev_store, check_mirror_bdev and
  * replace_mirror_replica (INTEGRATION.md 3c); two more, save_bdev_image and load_bdev_image, move any bdev's bytes to
- * and from a sparse image file (INTEGRATION.md 3d).
+ * and from a sparse image file, and three, enable_bdev_image_tracking, save_bdev_image_delta and
+ * apply_bdev_image_delta, move only what changed since the last image (INTEGRATION.md 3d).
  *
  * CLI as S/app/vhost/vhost.c:43-48 + S/lib/event/app.c:826-960:
  *   -S <dir> vhost socket directory   -r <path> RPC socket (default /var/tmp/spdk.sock)
@@ -603,6 +604,33 @@ static Reply dispatch(const std::string &method, const Json *params, const Json 
 				  ",\"block_size\":" + std::to_string(info.block_size) + ",\"num_blocks\":" + std::to_string(info.num_blocks) +
 				  ",\"uuid\":" + jstr(info.uuid) + ",\"extents\":" + std::to_string(info.nextents) +
 				  ",\"data_bytes\":" + std::to_string(info.data_bytes) + ",\"file_bytes\":" + std::to_string(info.file_bytes) + "}");
+	}
+	if (method == "enable_bdev_image_tracking") {
+		/* keep the fingerprints a delta is taken against; like the images, not part of the configuration dump */
+		if (!decode(params, {{"name", Json::Str, false, &a}, {"enable", Json::Bool, true, &b}})) return bad;
+		int rc = oimgpu_bdev_image_track(a->raw.c_str(), b ? b->b : 1);
+		if (rc < 0) return error(id, E_INVALID_PARAMS, strerr(rc));
+		return result(id, "true");
+	}
+	if (method == "save_bdev_image_delta" || method == "apply_bdev_image_delta") {
+		/* the granules a tracked bdev changed since its last save or load, to a new delta file; or a delta into a bdev
+		 * nothing has open yet whose content is the delta's parent */
+		if (!decode(params, {{"name", Json::Str, false, &a}, {"path", Json::Str, false, &b}})) return bad;
+		oimgpu_image_delta_info info;
+		int rc = method == "save_bdev_image_delta" ? oimgpu_bdev_image_save_delta(a->raw.c_str(), b->raw.c_str(), &info)
+							   : oimgpu_bdev_image_apply_delta(a->raw.c_str(), b->raw.c_str(), &info);
+		if (rc < 0) return error(id, E_INVALID_PARAMS, strerr(rc));
+		auto hex = [](const uint64_t d[2]) {
+			char s[33];
+			snprintf(s, sizeof(s), "%016llx%016llx", (unsigned long long)d[0], (unsigned long long)d[1]);
+			return jstr(s);
+		};
+		return result(id, "{\"name\":" + jstr(a->raw) + ",\"path\":" + jstr(b->raw) +
+				  ",\"block_size\":" + std::to_string(info.block_size) + ",\"num_blocks\":" + std::to_string(info.num_blocks) +
+				  ",\"uuid\":" + jstr(info.uuid) + ",\"extents\":" + std::to_string(info.nextents) +
+				  ",\"data_bytes\":" + std::to_string(info.data_bytes) + ",\"zero_bytes\":" + std::to_string(info.zero_bytes) +
+				  ",\"file_bytes\":" + std::to_string(info.file_bytes) + ",\"parent_digest\":" + hex(info.parent_digest) +
+				  ",\"digest\":" + hex(info.digest) + "}");
 	}
 	if (method == "delete_bdev") {
 		if (!decode(params, {{"name", Json::Str, false, &a}})) return bad;

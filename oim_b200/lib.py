@@ -73,6 +73,9 @@ SYMBOLS = [
     ("oimgpu_bdev_mirror_check", _I, [C.c_char_p, _U64, _U64, _I, _VP, _U32, _VP]),
     ("oimgpu_bdev_image_save", _I, [C.c_char_p, C.c_char_p, _VP]),
     ("oimgpu_bdev_image_load", _I, [C.c_char_p, C.c_char_p, _VP]),
+    ("oimgpu_bdev_image_track", _I, [C.c_char_p, _I]),
+    ("oimgpu_bdev_image_save_delta", _I, [C.c_char_p, C.c_char_p, _VP]),
+    ("oimgpu_bdev_image_apply_delta", _I, [C.c_char_p, C.c_char_p, _VP]),
     ("oimgpu_bdev_delete", _I, [C.c_char_p]),
     ("oimgpu_bdev_get", _I, [C.c_char_p, C.POINTER(BdevInfo)]),
     ("oimgpu_bdev_list", _I, [C.POINTER(BdevInfo), _I]),
@@ -303,6 +306,34 @@ def bdev_image_save(name: str, path) -> dict:
 def bdev_image_load(name: str, path) -> dict:
     """fill every replica of the unused bdev `name` from the image file `path` (include/oimgpu.h oimgpu_bdev_image_load)"""
     return _image_call(load().oimgpu_bdev_image_load, "bdev_image_load", name, path)
+
+
+def bdev_image_track(name: str, enable: bool = True) -> None:
+    """keep (or stop keeping) the fingerprint tables that let bdev `name`'s next save_delta write only the granules that
+    changed since its last save or load (include/oimgpu.h oimgpu_bdev_image_track)"""
+    _chk(load().oimgpu_bdev_image_track(_b(name), int(enable)), "bdev_image_track")
+
+
+def _delta_call(fn, what: str, name: str, path) -> dict:
+    out = np.zeros(1, dtype=abi.image_delta_info_dtype)
+    _chk(fn(_b(name), os.fsencode(path), out.ctypes.data), what)
+    o = out[0]
+    return {"num_blocks": int(o["num_blocks"]), "block_size": int(o["block_size"]), "granule_bytes": int(o["granule_bytes"]),
+            "nextents": int(o["nextents"]), "data_bytes": int(o["data_bytes"]), "zero_bytes": int(o["zero_bytes"]),
+            "file_bytes": int(o["file_bytes"]), "parent_digest": tuple(int(x) for x in o["parent_digest"]),
+            "digest": tuple(int(x) for x in o["digest"]), "uuid": bytes(o["uuid"]).split(b"\0", 1)[0].decode()}
+
+
+def bdev_image_save_delta(name: str, path) -> dict:
+    """write the granules of tracked bdev `name` that changed since its baseline to the new delta file `path`
+    (include/oimgpu.h oimgpu_bdev_image_save_delta)"""
+    return _delta_call(load().oimgpu_bdev_image_save_delta, "bdev_image_save_delta", name, path)
+
+
+def bdev_image_apply_delta(name: str, path) -> dict:
+    """apply the delta file `path` to every replica of the unused bdev `name`, whose content must be the delta's parent
+    (include/oimgpu.h oimgpu_bdev_image_apply_delta)"""
+    return _delta_call(load().oimgpu_bdev_image_apply_delta, "bdev_image_apply_delta", name, path)
 
 
 def delete_bdev(name: str) -> None:
